@@ -6,6 +6,8 @@ rank takes 32 pages of the round-robin shard, i.e. configs[2] at 8 GPUs; weak sc
   python bench.py --gpus N --steps K --warmup W                      # ours (hand-written CUDA through the C ABI)
   python bench.py --impl reference --gpus N --steps K --warmup W     # CPU restatement of the reference path (oracle/)
 
+  python bench.py ... --dump-outputs DIR     # also write what the timed path computed in its last step, as DIR/<name>.npy
+
 One JSON line on stdout (rank 0).  `value` = device-resident throughput (inputs staged in HBM, CUDA-event timed, max over
 ranks); `e2e` = the same pages through the plugin `infer` calls with pinned HOST buffers (H2D/D2H and host glue inside
 the timed region); `roofline` = dominant kernel class from per-launch CUDA events recorded during the timed region;
@@ -44,7 +46,7 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet (dense bf16, HBM3), not measured")
 
 
 def build_weights():
@@ -60,7 +62,7 @@ def build_weights():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled while the timed region runs (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons sampled while the timed region runs (read only: nothing is set)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -142,7 +144,7 @@ def run_reference(args, rank, world):
 
 # ----------------------------------------------------------------------------------------------------------------------
 # GPU bar (SURVEY 8d(2)): the same functional modules (oracle/nets.py, pinned against the reference nn.Modules) moved to the
-# B200 and run in eager PyTorch -> cuDNN / cuBLAS / cuFFT library kernels, N=1 per forward as the reference does
+# GPU and run in eager PyTorch -> cuDNN / cuBLAS / cuFFT library kernels, N=1 per forward as the reference does
 # (manga_translator.py:1491-1519), with the reference's own flags: allow_tf32 (manga_translator.py:133-138) and LaMa under
 # bf16 autocast (config.py:296-299, inpainting_lama_mpe.py:100-107); and once more in plain fp32.  Device-resident inputs,
 # CUDA-event timed, bilateral filter / contours / crops excluded (they are host code in the reference): this is the bar
@@ -409,6 +411,41 @@ def c4_figure(hp, n_pages):
             "uint8 in / uint8 out incl. pack, blend and composite; bottleneck 320x240x512, FFT 320x240"}
 
 
+DUMP_BYTES = 64 << 20          # --dump-outputs: at most this much in all
+DUMP_SAMPLE = 98304            # elements per page of each page-sized output (fixed, seeded positions)
+
+
+def dump_outputs(directory, results, rank):
+    """Write what the timed path returned for every page of its last step (`results` = [(page index, (db, dmask, ocr, out))]) as
+    float32 / float64 .npy files: the OCR results whole (entries past each line's kept count zeroed, they are unspecified), the
+    page-sized outputs (detector probability map and text mask, inpainted page) as a fixed seeded sample of DUMP_SAMPLE elements per
+    page.  Positions depend only on the page index and the output shape, so two builds run with the same arguments compare
+    element for element."""
+    os.makedirs(directory, exist_ok=True)
+    cols = {k: [] for k in ("db", "text_mask", "inpainted", "ocr_counts", "ocr_steps", "ocr_chars", "ocr_logprob", "ocr_colors")}
+    for page_index, (db, dmask, ocr, out) in results:
+        for name, t in (("db", db), ("text_mask", dmask), ("inpainted", out)):
+            flat = t.reshape(-1)
+            rng = np.random.default_rng(1000003 * page_index + flat.numel())
+            pos = np.sort(rng.choice(flat.numel(), size=min(DUMP_SAMPLE, flat.numel()), replace=False))
+            cols[name].append(flat[torch.from_numpy(pos).to(flat.device)].float().cpu().numpy())
+        for counts, steps, chars, lp, col in ocr:
+            keep = torch.arange(steps.shape[1], device=counts.device)[None, :] < counts[:, None].long()
+            cols["ocr_counts"].append(counts.double().cpu().numpy())
+            cols["ocr_steps"].append(torch.where(keep, steps, 0).double().cpu().numpy().reshape(-1))
+            cols["ocr_chars"].append(torch.where(keep, chars, 0).double().cpu().numpy().reshape(-1))
+            cols["ocr_logprob"].append(torch.where(keep, lp, 0.0).cpu().numpy().reshape(-1))
+            cols["ocr_colors"].append(torch.where(keep[..., None], col, 0.0).cpu().numpy().reshape(-1))
+    arrays = {k: np.concatenate(v) if v else np.zeros(0, np.float32) for k, v in cols.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_BYTES:
+        raise SystemExit(f"bench.py: --dump-outputs would write {total / 2**20:.1f} MB (limit {DUMP_BYTES >> 20} MB); run fewer pages")
+    suffix = f"_rank{rank}" if rank else ""
+    for k, a in arrays.items():
+        np.save(os.path.join(directory, k + suffix + ".npy"), a)
+    log(f"[bench] rank {rank}: {len(arrays)} arrays ({total / 2**20:.1f} MB) of the last timed step written to {directory}")
+
+
 def run_ours(args, rank, world, local_rank):
     import torch.distributed as dist
     from mit_b200 import exchange, synth
@@ -452,9 +489,11 @@ def run_ours(args, rank, world, local_rank):
     # multi-GPU: fixed-size result records (boxes, scores, OCR text / colours, raw mask, inpainted page) all-gathered over NCCL
     xchg = ResultExchange(dev, len(pages), PAGE_H, PAGE_W) if world > 1 else None
 
-    def resident_step():
+    def resident_step(keep=None):
         for i, sp in enumerate(staged):
             db, dmask, ocr, out = hp.run_resident(sp)
+            if keep is not None:                             # --dump-outputs: the results of the last timed step
+                keep.append((idxs[i], (db, dmask, ocr, out)))
             if xchg is not None:                             # N > 1: the page goes into this rank's result record, device to device
                 o, nb = xchg.lay.o["page"]
                 xchg.buf[i, o:o + nb].copy_(out.reshape(-1))
@@ -472,9 +511,10 @@ def run_ours(args, rank, world, local_rank):
         clocks.start()
     launches0 = eng.launches
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    last = [] if args.dump_outputs else None
     e0.record()
-    for _ in range(args.steps):
-        resident_step()
+    for step in range(args.steps):
+        resident_step(last if step == args.steps - 1 else None)
     e1.record()
     barrier()
     ms_total = max_over_ranks(e0.elapsed_time(e1))
@@ -483,6 +523,9 @@ def run_ours(args, rank, world, local_rank):
     prof = json.loads(eng.lib.mitb_profile_report(eng._h).decode())
     launch_list = prof.pop("_launches", [])               # per-launch conv list (MITB_PROFILE_LAUNCHES), not a kernel class
     eng.lib.mitb_profile_enable(eng._h, 0)
+    if last is not None:
+        dump_outputs(args.dump_outputs, last, rank)
+        del last
     value = args.steps * n_pages * world / (ms_total / 1e3)
     # the same region once more WITHOUT the per-launch event pairs of the profiler (they cost ~2 us per launch): informational
     barrier()
@@ -613,7 +656,11 @@ def main():
     ap.add_argument("--no-c4", action="store_true", help="skip the lama_large @ 2560 (BASELINE configs[3]) figure")
     ap.add_argument("--workers", type=int, default=8, help="host threads of the page pipeline in the e2e leg")
     ap.add_argument("--fast-e2e", action="store_true", help="one warm-up step for the e2e leg (development only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path computed in its last step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-/* libmitb -- C ABI of the B200-native detect -> OCR -> inpaint hot path.
+/* libmitb -- C ABI of the H100-native detect -> OCR -> inpaint hot path.
  *
  * Drop-in boundary for manga-image-translator's three dense-inference plugins.  Every entry point replaces the
  * torch call made by the reference at the cited line (paths relative to manga_translator/):
@@ -43,7 +43,7 @@ const char* mitb_version(void);
 long long mitb_launch_count(const mitb_ctx* ctx);      /* kernels launched by this context so far */
 size_t mitb_workspace_bytes(const mitb_ctx* ctx);      /* current activation workspace size */
 
-/* Process-wide switch between the tcgen05 (bf16x3 split, ~1e-5 relative) and the exact-fp32 SIMT convolution kernels.
+/* Process-wide switch between the wgmma (bf16x3 split, ~1e-5 relative) and the exact-fp32 SIMT convolution kernels.
  * Default on.  The SIMT kernels are the parity anchor of the tensor-core path (tests run both). */
 int mitb_set_tensor_cores(int on);
 /* LaMa FFC layer implementation (process-wide): 0 = generic planar path (any size), 1 = fused NHWC path (operand-fused GEMMs +

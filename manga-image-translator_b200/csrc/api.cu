@@ -36,7 +36,7 @@ static Weights collect(const mitb_tensor* w, int n) {
 
 extern "C" {
 
-const char* mitb_version(void) { return "mitb-b200 0.1 (sm_100a)"; }
+const char* mitb_version(void) { return "mitb-b200 0.1 (sm_90a)"; }
 
 int mitb_create(int device, mitb_ctx** out) {
   if (!out) return 1;
@@ -47,7 +47,8 @@ int mitb_create(int device, mitb_ctx** out) {
   if (device < 0 || device >= count) { g_create_error = "mitb_create: bad device ordinal"; return 3; }
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { g_create_error = "mitb_create: cudaGetDeviceProperties failed"; return 3; }
-  if (prop.major < 10) { g_create_error = std::string("mitb_create: ") + prop.name + " is not a Blackwell (sm_100a) device"; return 3; }
+  // the kernels are built for sm_90a only (wgmma, TMA): anything else cannot load them
+  if (prop.major != 9 || prop.minor != 0) { g_create_error = std::string("mitb_create: ") + prop.name + " is not a Hopper (sm_90a) device"; return 3; }
   mitb_ctx* c = new mitb_ctx();
   c->c.device = device;
   *out = c;

@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(BTX * BTY) bilateral17_kernel(const uint8_t* i
   // OpenCV's own implementation (bilateral_filter.simd.hpp) multiplies by the reciprocal: w = 1 / wsum; b = cvRound(sum_b * w).
   // This is bit-exact against cv2 with IPP disabled on every machine.  The stock pip wheel routes 8-bit bilateralFilter through
   // Intel IPP, a closed-source kernel whose rounding differs from OpenCV's own in a few bytes per million AND between CPUs
-  // (measured: per-channel division on one host, something else again on the B200 box), so it cannot serve as a definition.
+  // (per-channel division on one host, something else again on another), so it cannot serve as a definition.
   const float inv = __fdiv_rn(1.f, ws);
   uint8_t* o = out + ((size_t)y * W + x) * 3;
   o[0] = (uint8_t)__float2int_rn(__fmul_rn(s0, inv));

@@ -408,7 +408,7 @@ void launch_repack(float* dst, const float* src, int Cout, int Cin, int ntaps, c
   CUDA_OK(cudaMemcpyAsync(d, ky, sizeof(int) * ntaps, cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaMemcpyAsync(d + ntaps, kx, sizeof(int) * ntaps, cudaMemcpyHostToDevice, st));
   const long total = (long)ntaps * Cin * ldw;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
   repack_kernel<<<blocks, 256, 0, st>>>(dst, src, Cout, Cin, ntaps, d, d + ntaps, s_co, s_c, s_ky, s_kx, ldw);
   CUDA_OK(cudaGetLastError());
   CUDA_OK(cudaStreamSynchronize(st));

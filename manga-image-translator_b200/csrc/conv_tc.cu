@@ -1,28 +1,20 @@
-// tcgen05 (5th-gen tensor core) implicit-GEMM convolution for sm_100a, register-gather variant.
+// wgmma (Hopper warpgroup MMA) implicit-GEMM convolution for sm_90a, register-gather variant.
 //
 // Same contract as the SIMT kernel in conv_simt.cu (tap list, zero/reflect padding, strided output mapping for the
-// transposed-conv phases, BN+ReLU prologue, fused epilogue), contraction on the tensor cores.  Since r01 the main path is
-// conv_tma.cu (activations split once, every operand by TMA); this kernel keeps the layers that one does not take: inputs
-// whose channel count is not a multiple of 8 (Cin = 4 stems) and tiny-M / huge-K decoder layers that need split-K.
+// transposed-conv phases, BN+ReLU prologue, fused epilogue), contraction on the tensor cores.  The main path is conv_tma.cu
+// (activations split once, every operand by TMA); this kernel keeps the layers that one does not take: inputs whose channel
+// count is not a multiple of 8 and tiny-M / huge-K decoder layers that need split-K.
 //
-//   * 128-pixel x BN-channel output tile per CTA, accumulator in TMEM (128 lanes x BN fp32 columns, double buffered).
+//   * 128-pixel x BN-channel output tile per CTA, two warpgroups of 64 rows each, fp32 accumulators in registers.
 //   * fp32 accuracy from bf16 tensor cores by operand splitting ("bf16x3"): x = hi + mid with hi = bf16(x),
 //     mid = bf16(x - hi); D += A_hi*B_hi + A_hi*B_mid + A_mid*B_hi.  The dropped terms are <= ~3*2^-18 relative
-//     (about 1e-5), far inside the 1e-3 parity budget, at 1/3 of the bf16 tensor rate (2x a 3xTF32 scheme).
-//   * K is consumed in blocks of 64 (one 128-byte swizzle row of bf16).  Warp-specialised, 320 threads (168 registers: the
-//     register file is partitioned per SM sub-partition, three warps of 168 x 32 fit in its 16 K registers):
-//       warps 0-7  two ping-pong groups of 128 threads gather alternate K blocks of the activation tile from the NHWC view
-//                  (thread = one float4 column of 16 rows: a warp load covers two complete 256-byte row segments), apply the
-//                  optional BN+ReLU prologue, split hi/mid and store both tiles in the UMMA K-major SWIZZLE_128B layout;
-//                  planar (NCHW) inputs use a row-per-thread gather that is coalesced along pixels.  After the last K
-//                  block the same warps run the epilogue (tcgen05.ld, shared-memory transpose, (+add0)*scale+shift -> act ->
-//                  *mul1 -> +add1, coalesced fp32 stores, or row-stat / split-K partials);
-//       warp  9    one thread streams the pre-split K-major bf16 weight tiles (hi/mid) with TMA (cp.async.bulk.tensor,
-//                  128B swizzle) straight into the stage, completing on the stage's "full" mbarrier (expect_tx);
-//       warp  8    one thread issues tcgen05.mma (12 per K block) and commits to the stage's "empty" mbarrier;
-//     full/empty mbarrier ring, producers signal after fence.proxy.async (generic-proxy stores -> async-proxy reads).
+//     (about 1e-5), far inside the 1e-3 parity budget, at 1/3 of the bf16 tensor rate.
+//   * K is consumed in blocks of 64 (one 128-byte swizzle row of bf16), two shared-memory stages.  All 256 threads gather the
+//     activation block of the next stage from the NHWC view (thread = one float4 column of 8 rows; a warp load covers two
+//     complete 256-byte row segments) or the planar view (two threads per row, coalesced along pixels), apply the optional
+//     BN+ReLU prologue, split hi/mid and store both tiles in the K-major SWIZZLE_128B layout, while the wgmma of the previous
+//     block runs; thread 0 streams the pre-split K-major bf16 weight tiles (hi/mid) with TMA onto the stage's mbarrier.
 //   * Persistent: one CTA per SM loops over output tiles; split-K (splitk_reduce_kernel) when tiles cannot fill the SMs.
-//   Measured limit (profiles/r01_tc_skeleton_experiments.txt): the producers' own instruction stream, ~160 TF/s.
 #include <cuda.h>
 #include <string.h>
 #include <cuda_bf16.h>
@@ -33,9 +25,9 @@ namespace mitb {
 namespace {
 
 constexpr int TC_BM = 128, TC_BK = 64;
-constexpr int TC_AWARPS = 8;                  // A-producer warps; they also run the epilogue of the tile they just produced
-constexpr int TC_MMAWARP = TC_AWARPS, TC_TMAWARP = TC_AWARPS + 1;
-constexpr int TC_THREADS = (TC_AWARPS + 2) * 32;   // 320 threads -> up to 204 registers per thread, no spills
+constexpr int TC_THREADS = 256;              // two warpgroups: gather + wgmma + epilogue
+
+#include "tc_common.cuh"
 
 struct TcParams {
   const float* in; int N, H, W, in_cs, in_coff, Cin, in_planar;
@@ -43,233 +35,60 @@ struct TcParams {
   int kpad, npad;                                             // weights [npad][kpad] bf16, K-major, zero padded
   int ntaps; int8_t tdy[kMaxTaps], tdx[kMaxTaps];
   int sy, sx, pad, Ho, Wo;
-  float* out; int oH, oW, out_cs, out_coff, Cout, out_planar, oy_mul, oy_add, ox_mul, ox_add;
   const float* in_scale; const float* in_shift; int in_relu;
-  const float* add0; int add0_cs, add0_coff, add0_planar;
-  const float* add1; int add1_cs, add1_coff, add1_planar;
-  const float* scale; const float* shift; const float* mul1; int act;
-  float* stat_max; float* stat_sum; int* stat_idx; int stat_ld;     // fused log-softmax/argmax partials (vocabulary head)
-  int M, K, BN, stages, tmem_cols;
-  int splits; float* partial;                                       // split-K: partial sums [splits][M][npad]
-  int tmin_dy, tmax_dy, tmin_dx, tmax_dx;                           // extent of the tap offsets (fast interior addressing)
+  int M, K, splits;
+  int tmin_dy, tmax_dy, tmin_dx, tmax_dx;                     // extent of the tap offsets (fast interior addressing)
+  EpiParams e;
 };
 
-#include "tc_common.cuh"
-
-template <int ACT>
+template <int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stage][A_hi 16K | A_mid 16K | B_hi BN*128 | B_mid BN*128], then barriers
+  // carve: [stage 0, 1][A_hi 16K | A_mid 16K | B_hi BN*128 | B_mid BN*128], then the two "full" barriers
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int BN = p.BN, S = p.stages;
-  const uint32_t a_bytes = TC_BM * 128, b_bytes = (uint32_t)BN * 128;
-  const uint32_t stage_bytes = 2 * a_bytes + 2 * b_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);   // full[S], empty[S], tfull[2], tempty[2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 4);
-  float* estage = reinterpret_cast<float*>(bars + 2 * S + 6);          // [TC_AWARPS][32 rows][20 floats] epilogue transpose buffer
+  constexpr uint32_t a_bytes = TC_BM * 128, b_bytes = (uint32_t)BN * 128;
+  constexpr uint32_t stage_bytes = 2 * a_bytes + 2 * b_bytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar_base = smem_u32(bars);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (2 * S + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (2 * S + 2 + b); };
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int nkb = p.kpad / TC_BK;
   const int mt = (p.M + TC_BM - 1) / TC_BM, nt = p.npad / BN;
   const int total_tiles = mt * nt * p.splits;
-  const uint32_t acc_stride = (uint32_t)(p.tmem_cols >> 1);          // columns per accumulator buffer
+  const int HoWo = p.Ho * p.Wo;
 
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), (p.in_planar ? TC_AWARPS * 32 : TC_AWARPS * 16) + 1); mbar_init(empty_bar(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tfull_bar(b), 1); mbar_init(tempty_bar(b), TC_AWARPS * 32); }
+    for (int s = 0; s < 2; ++s) mbar_init(full_bar(s), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == TC_MMAWARP) tmem_alloc(smem_u32(tmem_slot), (uint32_t)p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // tile t -> (split z, M tile, N tile); N fastest so CTAs running together share the activation rows in L2
-  auto decode = [&](int t, int& z, int& m0, int& n0, int& kb_begin, int& kb_end) {
-    z = t / (mt * nt); const int r = t - z * (mt * nt);
-    m0 = (r / nt) * TC_BM; n0 = (r % nt) * BN;
-    kb_begin = (int)(((long)z * nkb) / p.splits); kb_end = (int)(((long)(z + 1) * nkb) / p.splits);
-  };
+  // NHWC gather: thread owns float4 column f4 of the 8 rows rb + 16 i (same swizzle phase, 2048 B apart)
+  const int f4 = tid & 15, rb = tid >> 4;
+  const uint32_t soff0 = (uint32_t)rb * 128u + ((((uint32_t)f4 >> 1) ^ ((uint32_t)rb & 7u)) << 4) + ((uint32_t)f4 & 1u) * 8u;
+  // planar gather: two threads per GEMM row, 32 k each
+  const int pr = tid & 127, phalf = tid >> 7;
+  const uint32_t prow_off = (uint32_t)pr * 128u, psw = (uint32_t)(pr & 7);
 
-// ---- epilogue of one tile, run by the 8 producer warps: warp w reads TMEM lane quarter (w & 3) and the column half (w >> 2)
-  auto epilogue_tile = [&](int lt, int z, int m0, int n0) {
-    const int q = warp & 3, ehalf = warp >> 2;
-    const int r = q * 32 + lane;
-    const int HoWo = p.Ho * p.Wo;
-    const int buf = lt & 1;
-    const int m = m0 + r;
-    const bool row_ok = m < p.M;
-    const int nchunks = BN / 16, h0 = (nchunks + 1) / 2;
-    const int cb_lo = (ehalf == 0 ? 0 : h0) * 16, cb_hi = (ehalf == 0 ? h0 : nchunks) * 16;
-    mbar_wait(tfull_bar(buf), (lt >> 1) & 1);
-    tc_fence_after();
-    const uint32_t taddr_row = tmem_base + (uint32_t)buf * acc_stride + ((uint32_t)(q * 32) << 16);
-    if (p.stat_max) {
-      // vocabulary head: online (max, first argmax, sum exp) over this thread's columns of its row; the logits never leave
-      // TMEM (model_48px_ctc.py:460-461).  Two partials per N tile (one per column half).
-      float bm = -INFINITY, bs = 0.f; int bi = 0x7fffffff;
-#pragma unroll 1
-      for (int cb = cb_lo; cb < cb_hi; cb += 16) {
-        uint32_t raw[16];
-        tmem_ld16(taddr_row + (uint32_t)cb, raw);
-        tmem_ld_wait();
+  int it = 0;                                      // global K-block counter of this CTA (stage = it & 1)
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    // tile t -> (split z, M tile, N tile); N fastest so CTAs running together share the activation rows in L2
+    const int z = t / (mt * nt), rr0 = t - z * (mt * nt);
+    const int m0 = (rr0 / nt) * TC_BM, n0 = (rr0 % nt) * BN;
+    const int kb_begin = (int)(((long)z * nkb) / p.splits), kb_end = (int)(((long)(z + 1) * nkb) / p.splits);
+
+    // ---- NHWC row setup: pointer to the pixel under tap (0,0) and its (iy0, ix0); rows whose whole tap window lies inside the
+    // image take the fast address path (pointer + per-K-block tap offset), border rows redo the padded index arithmetic
+    uint32_t roff[8]; int ryx[8]; uint32_t okmask = 0, imask = 0;     // element offsets fit 32 bits (checked on the host)
+    int tap = 0, ci = 0;
+    // ---- planar row setup
+    int pnimg = 0, ppix = 0; bool prow_ok = false;
+    if (!p.in_planar) {
 #pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int c = n0 + cb + e;
-          if (c < p.Cout) {
-            const float x = __uint_as_float(raw[e]) + (p.shift ? __ldg(p.shift + c) : 0.f);
-            if (x > bm) { bs = bs * expf(bm - x) + 1.f; bm = x; bi = c; }
-            else bs += expf(x - bm);
-          }
-        }
-      }
-      if (row_ok) {
-        const size_t o = (size_t)m * p.stat_ld + (n0 / BN) * 2 + ehalf;
-        p.stat_max[o] = bm; p.stat_sum[o] = bs; p.stat_idx[o] = bi;
-      }
-    } else if (p.splits > 1) {
-      // split-K partial: raw accumulators to partial[z][m][npad]
-      float* dst = p.partial + ((size_t)z * p.M + m) * p.npad + n0;
-#pragma unroll 1
-      for (int cb = cb_lo; cb < cb_hi; cb += 16) {
-        uint32_t raw[16];
-        tmem_ld16(taddr_row + (uint32_t)cb, raw);
-        tmem_ld_wait();
-        if (row_ok) {
-#pragma unroll
-          for (int qq = 0; qq < 4; ++qq)
-            *reinterpret_cast<uint4*>(dst + cb + qq * 4) = make_uint4(raw[qq * 4], raw[qq * 4 + 1], raw[qq * 4 + 2], raw[qq * 4 + 3]);
-        }
-      }
-    } else if (!p.out_planar && ((p.out_cs | p.out_coff) & 3) == 0 &&
-               (!p.add0 || (!p.add0_planar && ((p.add0_cs | p.add0_coff) & 3) == 0)) &&
-               (!p.add1 || (!p.add1_planar && ((p.add1_cs | p.add1_coff) & 3) == 0))) {
-      // ---- NHWC output: transpose 32x16 accumulator chunks through shared memory so that one warp instruction touches
-      // 8 rows x 64 contiguous bytes (residual reads and stores coalesced) instead of 32 scattered 16-byte pieces
-      float* st = estage + (size_t)warp * 32 * 20;
-      const int sub = lane & 3, rsel = lane >> 2;              // this thread: columns 4*sub..+3 of rows rsel + 8j
-      size_t orow[4]; uint32_t rmask = 0;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int mm = m0 + q * 32 + rsel + 8 * j;
-        orow[j] = 0;
-        if (mm < p.M) {
-          const int ni = mm / HoWo, pp = mm - ni * HoWo;
-          orow[j] = ((size_t)ni * p.oH + (pp / p.Wo) * p.oy_mul + p.oy_add) * p.oW + (pp % p.Wo) * p.ox_mul + p.ox_add;
-          rmask |= 1u << j;
-        }
-      }
-#pragma unroll 1
-      for (int cb = cb_lo; cb < cb_hi; cb += 16) {
-        uint32_t raw[16];
-        tmem_ld16(taddr_row + (uint32_t)cb, raw);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          *reinterpret_cast<uint4*>(st + lane * 20 + 4 * i) = make_uint4(raw[4 * i], raw[4 * i + 1], raw[4 * i + 2], raw[4 * i + 3]);
-        __syncwarp();
-        const int cq = n0 + cb + 4 * sub;
-        if (cq < p.Cout) {
-          const bool full = cq + 3 < p.Cout;
-          float sc4[4] = {1.f, 1.f, 1.f, 1.f}, sh4[4] = {0.f, 0.f, 0.f, 0.f}, mu4[4] = {1.f, 1.f, 1.f, 1.f};
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            if (cq + e < p.Cout) {
-              if (p.scale) sc4[e] = __ldg(p.scale + cq + e);
-              if (p.shift) sh4[e] = __ldg(p.shift + cq + e);
-              if (p.mul1) mu4[e] = __ldg(p.mul1 + cq + e);
-            }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (!((rmask >> j) & 1u)) continue;
-            const float4 a = *reinterpret_cast<const float4*>(st + (rsel + 8 * j) * 20 + 4 * sub);
-            float v4[4] = {a.x, a.y, a.z, a.w};
-            if (p.add0) {
-              if (full) { const float4 tt = *reinterpret_cast<const float4*>(p.add0 + orow[j] * p.add0_cs + p.add0_coff + cq);
-                          v4[0] += tt.x; v4[1] += tt.y; v4[2] += tt.z; v4[3] += tt.w; }
-              else { for (int e = 0; e < 4; ++e) if (cq + e < p.Cout) v4[e] += p.add0[orow[j] * p.add0_cs + p.add0_coff + cq + e]; }
-            }
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              float x = v4[e];
-              if (p.scale) x *= sc4[e];
-              x += sh4[e];
-              x = act_t<ACT>(x, p.act);
-              if (p.mul1) x *= mu4[e];
-              v4[e] = x;
-            }
-            if (p.add1) {
-              if (full) { const float4 tt = *reinterpret_cast<const float4*>(p.add1 + orow[j] * p.add1_cs + p.add1_coff + cq);
-                          v4[0] += tt.x; v4[1] += tt.y; v4[2] += tt.z; v4[3] += tt.w; }
-              else { for (int e = 0; e < 4; ++e) if (cq + e < p.Cout) v4[e] += p.add1[orow[j] * p.add1_cs + p.add1_coff + cq + e]; }
-            }
-            if (full) *reinterpret_cast<float4*>(p.out + orow[j] * p.out_cs + p.out_coff + cq) = make_float4(v4[0], v4[1], v4[2], v4[3]);
-            else { for (int e = 0; e < 4; ++e) if (cq + e < p.Cout) p.out[orow[j] * p.out_cs + p.out_coff + cq + e] = v4[e]; }
-          }
-        }
-        __syncwarp();
-      }
-    } else {
-      // ---- planar (NCHW) or unaligned output: lane = pixel, so each channel's stores are already contiguous across lanes
-      int nimg = 0, pix = 0;
-      if (row_ok) { nimg = m / HoWo; pix = m - nimg * HoWo; }
-      const int py = (pix / p.Wo) * p.oy_mul + p.oy_add, px = (pix % p.Wo) * p.ox_mul + p.ox_add;
-      const size_t opix = ((size_t)nimg * p.oH + py) * p.oW + px;
-      const size_t oplane = (size_t)p.oH * p.oW, opl_pix = (size_t)py * p.oW + px;
-#pragma unroll 1
-      for (int cb = cb_lo; cb < cb_hi; cb += 16) {
-        uint32_t raw[16];
-        tmem_ld16(taddr_row + (uint32_t)cb, raw);
-        tmem_ld_wait();
-        if (!row_ok) continue;
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int c = n0 + cb + e;
-          if (c >= p.Cout) break;
-          float x = __uint_as_float(raw[e]);
-          if (p.add0) x += p.add0_planar ? p.add0[((size_t)nimg * p.add0_cs + p.add0_coff + c) * oplane + opl_pix] : p.add0[opix * p.add0_cs + p.add0_coff + c];
-          if (p.scale) x *= __ldg(p.scale + c);
-          if (p.shift) x += __ldg(p.shift + c);
-          x = act_t<ACT>(x, p.act);
-          if (p.mul1) x *= __ldg(p.mul1 + c);
-          if (p.add1) x += p.add1_planar ? p.add1[((size_t)nimg * p.add1_cs + p.add1_coff + c) * oplane + opl_pix] : p.add1[opix * p.add1_cs + p.add1_coff + c];
-          if (p.out_planar) p.out[((size_t)nimg * p.out_cs + p.out_coff + c) * oplane + opl_pix] = x;
-          else p.out[opix * p.out_cs + p.out_coff + c] = x;
-        }
-      }
-    }
-    tc_fence_before();
-    mbar_arrive(tempty_bar(buf));                       // accumulator drained -> the MMA warp may overwrite it
-  };
-  if (warp < TC_AWARPS && !p.in_planar) {
-    // =========================== A producers, NHWC input (coalesced, ping-pong groups) ===========================
-    // A K block is 64 channels = 16 float4 per GEMM row.  The 8 producer warps form two groups of 128 threads that take
-    // alternate K blocks: while one group splits/stores its block (and executes the proxy fence, which drains that
-    // thread's outstanding loads), the other group's global loads for the next block are in flight.  Inside a group thread
-    // tg owns float4 column f4 = tg&15 of the 16 rows rb+8i (rb = tg>>4): a warp instruction reads two complete 256-byte
-    // row segments, and all 16 loads of a thread share one (tap, channel) cursor.
-    const int grp = warp >> 2, tg = tid & 127;
-    const int f4 = tg & 15, rb = tg >> 4;
-    const int HoWo = p.Ho * p.Wo;
-    const uint32_t soff0 = (uint32_t)rb * 128u + ((((uint32_t)f4 >> 1) ^ ((uint32_t)rb & 7u)) << 4) + ((uint32_t)f4 & 1u) * 8u;
-    float4 v[16];
-    int git = 0, lt = 0;                               // global K-block / tile counters of this CTA
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
-      int z, m0, n0, kb_begin, kb_end;
-      decode(t, z, m0, n0, kb_begin, kb_end);
-      // per row: pointer to the pixel under tap (0,0) and its (iy0, ix0); rows whose whole tap window lies inside the
-      // image take the fast address path (pointer + per-K-block tap offset), border rows redo the padded index arithmetic
-      uint32_t roff[16]; int ryx[16]; uint32_t okmask = 0, imask = 0;     // element offsets fit 32 bits (checked on the host)
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int m = m0 + rb + 8 * i;
+      for (int i = 0; i < 8; ++i) {
+        const int m = m0 + rb + 16 * i;
         ryx[i] = 0; roff[i] = 0;
         if (m < p.M) {
           const int nimg = m / HoWo, rr = m - nimg * HoWo;
@@ -281,20 +100,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
           if (iy0 + p.tmin_dy >= 0 && iy0 + p.tmax_dy < p.H && ix0 + p.tmin_dx >= 0 && ix0 + p.tmax_dx < p.W) imask |= 1u << i;
         }
       }
-      // this group's first K block of the tile: the one whose global index has parity grp
-      int kb = kb_begin + ((grp - (git & 1)) & 1);
-      int tap, ci;
-      { const int k0 = kb * TC_BK + f4 * 4; tap = k0 / p.Cin; ci = k0 - tap * p.Cin; }
-      uint32_t valid = 0; int cur_ci = 0;
+      const int k0 = kb_begin * TC_BK + f4 * 4; tap = k0 / p.Cin; ci = k0 - tap * p.Cin;
+    } else {
+      const int m = m0 + pr;
+      prow_ok = m < p.M;
+      if (prow_ok) { pnimg = m / HoWo; ppix = m - pnimg * HoWo; }
+    }
 
-      auto load_block = [&](int kbl) {
+    float4 v[8]; uint32_t valid = 0; int cur_ci = 0;   // NHWC block in flight
+    float pv[4][8]; int pk = 0;                        // planar block in flight
+    auto load_block = [&](int kbl) {
+      if (!p.in_planar) {
         const int k = kbl * TC_BK + f4 * 4;
         cur_ci = ci; valid = 0;
         const bool kval = k < p.K;
         const int dy = kval ? p.tdy[tap] : 0, dx = kval ? p.tdx[tap] : 0;
         const int toff = (dy * p.W + dx) * p.in_cs + ci;
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
+        for (int i = 0; i < 8; ++i) {
           v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
           if (kval && ((imask >> i) & 1u)) {
             v[i] = __ldg(reinterpret_cast<const float4*>(p.in + (roff[i] + (uint32_t)toff)));
@@ -311,22 +134,29 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             }
           }
         }
-        ci += 2 * TC_BK; while (ci >= p.Cin) { ci -= p.Cin; ++tap; }      // this group's next block is two K blocks ahead
-      };
-
-      if (kb < kb_end) load_block(kb);
-      for (; kb < kb_end; kb += 2) {
-        const int itg = git + (kb - kb_begin);               // global index of this K block
-        const int s = itg % S;
+        ci += TC_BK; while (ci >= p.Cin) { ci -= p.Cin; ++tap; }
+      } else {
+        pk = kbl * TC_BK + phalf * 32;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int k = pk + j * 8;
+#pragma unroll
+          for (int e = 0; e < 8; ++e)
+            pv[j][e] = (prow_ok && k + e < p.K) ? __ldg(p.in + ((size_t)pnimg * p.in_cs + p.in_coff + k + e) * ((size_t)p.H * p.W) + ppix) : 0.f;
+        }
+      }
+    };
+    // BN+ReLU prologue (padding stays 0 after the transform) + hi/mid split + swizzled stores into stage s
+    auto store_block = [&](int s) {
+      uint8_t* a_hi = smem + (size_t)s * stage_bytes;
+      uint8_t* a_mid = a_hi + a_bytes;
+      if (!p.in_planar) {
         float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
         if (p.in_scale && valid) {
           sc = __ldg(reinterpret_cast<const float4*>(p.in_scale + cur_ci)); sh = __ldg(reinterpret_cast<const float4*>(p.in_shift + cur_ci));
         }
-        mbar_wait(empty_bar(s), ((itg / S) & 1) ^ 1);
-        uint8_t* a_hi = smem + (size_t)s * stage_bytes;
-        uint8_t* a_mid = a_hi + a_bytes;
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
+        for (int i = 0; i < 8; ++i) {
           float4 x = v[i];
           if (p.in_scale && ((valid >> i) & 1u)) {
             x.x = x.x * sc.x + sh.x; x.y = x.y * sc.y + sh.y; x.z = x.z * sc.z + sh.z; x.w = x.w * sc.w + sh.w;
@@ -334,179 +164,77 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
           }
           uint2 hi, mid;
           split4(x, hi, mid);
-          const uint32_t off = soff0 + (uint32_t)i * 1024u;          // row rb+8i: same swizzle phase, 8 rows further
+          const uint32_t off = soff0 + (uint32_t)i * 2048u;
           *reinterpret_cast<uint2*>(a_hi + off) = hi;
           *reinterpret_cast<uint2*>(a_mid + off) = mid;
         }
-        fence_async_smem();                                  // also drains this thread's loads: none are outstanding here
-        mbar_arrive(full_bar(s));
-        if (kb + 2 < kb_end) load_block(kb + 2);             // in flight while the other group produces the next K block
+      } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int k = pk + j * 8;
+          if (p.in_scale && prow_ok) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+              if (k + e < p.K) {
+                const float tt = pv[j][e] * __ldg(p.in_scale + k + e) + __ldg(p.in_shift + k + e);
+                pv[j][e] = p.in_relu ? fmaxf(tt, 0.f) : tt;
+              }
+          }
+          uint4 hi, mid;
+          split8(pv[j], hi, mid);
+          const uint32_t off = prow_off + ((((uint32_t)(phalf * 4 + j)) ^ psw) << 4);
+          *reinterpret_cast<uint4*>(a_hi + off) = hi;
+          *reinterpret_cast<uint4*>(a_mid + off) = mid;
+        }
       }
-      git += kb_end - kb_begin;
-      epilogue_tile(lt, z, m0, n0);
-    }
-  } else if (warp < TC_AWARPS) {
-    // =========================== A producers, planar input: two threads per GEMM row (coalesced along pixels) ===========
-    const int r = tid & 127, half = tid >> 7;
-    const int HoWo = p.Ho * p.Wo, HW = p.H * p.W;
-    const uint32_t row_off = (uint32_t)r * 128u;
-    const uint32_t sw = (uint32_t)(r & 7);
-    struct Blk { float v[4][8]; int cix[4]; };        // raw loaded values + channel index of each chunk (-1: all zero)
-    Blk R0, R1;
-    int it = 0, lt = 0;                                // global K-block / tile counters of this CTA
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
-      int z, m0, n0, kb_begin, kb_end;
-      decode(t, z, m0, n0, kb_begin, kb_end);
-      const int m = m0 + r;
-      const bool row_ok = m < p.M;
-      int nimg = 0, iy0 = 0, ix0 = 0, pix = 0;
-      if (row_ok) {
-        nimg = m / HoWo; const int rr = m - nimg * HoWo;
-        const int oy = rr / p.Wo, ox = rr - oy * p.Wo;
-        iy0 = oy * p.sy; ix0 = ox * p.sx; pix = rr;
-      }
-      int tap = 0, ci = 0;                             // cursor of this thread's next 8-channel chunk
-      if (!p.in_planar) { const int k0 = kb_begin * TC_BK + half * 32; tap = k0 / p.Cin; ci = k0 - tap * p.Cin; }
+    };
 
-      auto load_block = [&](int kb, Blk& B) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int k = kb * TC_BK + half * 32 + j * 8;
-#pragma unroll
-          for (int e = 0; e < 8; ++e) B.v[j][e] = 0.f;
-          B.cix[j] = -1;
-          if (row_ok && k < p.K) {
-            if (!p.in_planar) {
-              int iy = iy0 + p.tdy[tap], ix = ix0 + p.tdx[tap];
-              bool inb = true;
-              if (p.pad == PAD_REFLECT) { iy = reflect_tc(iy, p.H); ix = reflect_tc(ix, p.W); }
-              else inb = (iy >= 0) & (iy < p.H) & (ix >= 0) & (ix < p.W);
-              if (inb) {
-                const float* src = p.in + ((size_t)(nimg * p.H + iy) * p.W + ix) * p.in_cs + p.in_coff + ci;
-                const float4 a = __ldg(reinterpret_cast<const float4*>(src)), b = __ldg(reinterpret_cast<const float4*>(src) + 1);
-                B.v[j][0] = a.x; B.v[j][1] = a.y; B.v[j][2] = a.z; B.v[j][3] = a.w;
-                B.v[j][4] = b.x; B.v[j][5] = b.y; B.v[j][6] = b.z; B.v[j][7] = b.w;
-                B.cix[j] = ci;
-              }
-            } else {
-              B.cix[j] = k;
-#pragma unroll
-              for (int e = 0; e < 8; ++e)
-                if (k + e < p.K) B.v[j][e] = __ldg(p.in + ((size_t)nimg * p.in_cs + p.in_coff + k + e) * HW + pix);
-            }
-          }
-          if (!p.in_planar) { ci += 8; while (ci >= p.Cin) { ci -= p.Cin; ++tap; } }
-        }
-        if (!p.in_planar) { ci += 32; while (ci >= p.Cin) { ci -= p.Cin; ++tap; } }     // skip the other half-row
-      };
-      // BN+ReLU prologue (applied at consume time so the loads stay in flight) + hi/mid split + swizzled stores
-      auto produce = [&](int kb, Blk& B) {
-        const int s = it % S;
-        uint4 hi[4], mid[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if (p.in_scale && B.cix[j] >= 0) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const int ch = B.cix[j] + e;
-              if (!p.in_planar || ch < p.K) {
-                const float tt = B.v[j][e] * __ldg(p.in_scale + ch) + __ldg(p.in_shift + ch);
-                B.v[j][e] = p.in_relu ? fmaxf(tt, 0.f) : tt;
-              }
-            }
-          }
-          split8(B.v[j], hi[j], mid[j]);
-        }
-        if (kb + 2 < kb_end) load_block(kb + 2, B);     // refill this ring slot: loads stay in flight for two K blocks
-        mbar_wait(empty_bar(s), ((it / S) & 1) ^ 1);
-        uint8_t* a_hi = smem + (size_t)s * stage_bytes;
-        uint8_t* a_mid = a_hi + a_bytes;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint32_t c = (uint32_t)(half * 4 + j);
-          const uint32_t off = row_off + ((c ^ sw) << 4);
-          *reinterpret_cast<uint4*>(a_hi + off) = hi[j];
-          *reinterpret_cast<uint4*>(a_mid + off) = mid[j];
-        }
-        fence_async_smem();
-        mbar_arrive(full_bar(s));
-        ++it;
-      };
-      load_block(kb_begin, R0);
-      if (kb_begin + 1 < kb_end) load_block(kb_begin + 1, R1);
-      for (int kb = kb_begin; kb < kb_end; kb += 2) {
-        produce(kb, R0);
-        if (kb + 1 < kb_end) produce(kb + 1, R1);
+    float acc[BN / 2];
+    load_block(kb_begin);
+    for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
+      const int s = it & 1;
+      wgmma_wait<1>();                                 // this warp's MMAs of block it-2 (the last reader of stage s) are done
+      __syncthreads();                                 // ... and every other warp's
+      if (tid == 0) {
+        mbar_arrive_expect_tx(full_bar(s), 2 * b_bytes);
+        const uint32_t b_hi = smem_base + (uint32_t)s * stage_bytes + 2 * a_bytes;
+        tma_load_2d(b_hi, &p.tmh, full_bar(s), kb * TC_BK, n0);
+        tma_load_2d(b_hi + b_bytes, &p.tmm, full_bar(s), kb * TC_BK, n0);
       }
-      epilogue_tile(lt, z, m0, n0);
+      store_block(s);
+      fence_async_smem();                              // generic-proxy stores -> async-proxy (wgmma) reads
+      if (kb + 1 < kb_end) load_block(kb + 1);         // in flight while this block is multiplied
+      __syncthreads();
+      mbar_wait(full_bar(s), (it >> 1) & 1);
+      const uint32_t a_hi = smem_base + (uint32_t)s * stage_bytes + (uint32_t)wg * (64u * 128u), a_mid = a_hi + a_bytes;
+      const uint32_t b_hi = smem_base + (uint32_t)s * stage_bytes + 2 * a_bytes, b_mid = b_hi + b_bytes;
+      fence_acc(acc);
+      wgmma_fence();
+      wgmma_kblock_x3<BN>(acc, make_desc_sw128(a_hi), make_desc_sw128(a_mid), make_desc_sw128(b_hi), make_desc_sw128(b_mid), kb == kb_begin);
+      wgmma_commit();
+      fence_acc(acc);
     }
-  } else if (warp == TC_MMAWARP) {
-    // =========================== MMA issuer (one elected thread) ===========================
-    if (lane == 0) {
-      // instruction descriptor: D=F32 (bits 4-5 = 1), A=B=BF16 (bits 7-9 / 10-12 = 1), K-major A and B,
-      // N>>3 at bits 17-22, M>>4 at bits 24-28
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-      int it = 0, lt = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
-        int z, m0, n0, kb_begin, kb_end;
-        decode(t, z, m0, n0, kb_begin, kb_end);
-        const int buf = lt & 1;
-        mbar_wait(tempty_bar(buf), ((lt >> 1) & 1) ^ 1);             // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)buf * acc_stride;
-        for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
-          const int s = it % S;
-          mbar_wait(full_bar(s), (it / S) & 1);
-          tc_fence_after();
-          const uint32_t a_hi = smem_base + (uint32_t)s * stage_bytes, a_mid = a_hi + a_bytes;
-          const uint32_t b_hi = a_mid + a_bytes, b_mid = b_hi + b_bytes;
-          const uint64_t dah = make_desc_sw128(a_hi), dam = make_desc_sw128(a_mid), dbh = make_desc_sw128(b_hi), dbm = make_desc_sw128(b_mid);
-#pragma unroll
-          for (int j = 0; j < TC_BK / 16; ++j) {
-            const uint64_t adv = (uint64_t)(j * 2);                  // 16 bf16 = 32 bytes = 2 x 16-byte units inside the swizzle row
-            umma_bf16(tmem_d, dah + adv, dbh + adv, idesc, (kb > kb_begin || j > 0) ? 1u : 0u);
-            umma_bf16(tmem_d, dah + adv, dbm + adv, idesc, 1u);
-            umma_bf16(tmem_d, dam + adv, dbh + adv, idesc, 1u);
-          }
-          umma_commit(empty_bar(s));          // implies tcgen05.fence::before_thread_sync; frees the stage when the MMAs retire
-        }
-        umma_commit(tfull_bar(buf));          // accumulator of this tile complete -> epilogue
-      }
-    }
-    __syncwarp();
-  } else if (warp == TC_TMAWARP) {
-    // =========================== B producer: TMA of the pre-split K-major bf16 weight tiles ===========================
-    if (lane == 0) {
-      int it = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-        int z, m0, n0, kb_begin, kb_end;
-        decode(t, z, m0, n0, kb_begin, kb_end);
-        for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
-          const int s = it % S;
-          mbar_wait(empty_bar(s), ((it / S) & 1) ^ 1);
-          const uint32_t b_hi = smem_base + (uint32_t)s * stage_bytes + 2 * a_bytes, b_mid = b_hi + b_bytes;
-          mbar_arrive_expect_tx(full_bar(s), 2 * b_bytes);
-          tma_load_2d(b_hi, &p.tmh, full_bar(s), kb * TC_BK, n0);
-          tma_load_2d(b_mid, &p.tmm, full_bar(s), kb * TC_BK, n0);
-        }
-      }
-    }
-    __syncwarp();
+    wgmma_wait<0>();
+    fence_acc(acc);
+    epilogue_tile<-1, BN>(p.e, acc, wg * 64 + (warp & 3) * 16 + (lane >> 2), n0, z, [&](int r, int& nimg, int& oy, int& ox) -> bool {
+      const int m = m0 + r;
+      if (m >= p.M) return false;
+      nimg = m / HoWo; const int pp = m - nimg * HoWo;
+      oy = pp / p.Wo; ox = pp - oy * p.Wo;
+      return true;
+    });
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == TC_MMAWARP) { tc_fence_after(); tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols); }
 }
 
 // split-K second pass: sum the partials and run the regular epilogue (one thread per 4 output channels of a pixel)
-__global__ void __launch_bounds__(256) splitk_reduce_kernel(const __grid_constant__ TcParams p) {
+__global__ void __launch_bounds__(256) splitk_reduce_kernel(const __grid_constant__ EpiParams p, int splits) {
   const int nq = (p.Cout + 3) / 4;
   const long total = (long)p.M * nq;
   const int HoWo = p.Ho * p.Wo;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int m = (int)(i / nq), cq = (int)(i - (long)m * nq) * 4;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int z = 0; z < p.splits; ++z) {
+    for (int z = 0; z < splits; ++z) {
       const float4 t = *reinterpret_cast<const float4*>(p.partial + ((size_t)z * p.M + m) * p.npad + cq);
       acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
     }
@@ -558,11 +286,13 @@ __global__ void split_weights_padded_kernel(const float* w, int ntaps, int Cin, 
   }
 }
 
+// N tile of the weight copies (and of the row-stat layout): at most 128 columns (64 fp32 accumulator registers per thread of a
+// warpgroup), a multiple of 32 (the wgmma widths instantiated)
 int pick_bn(int Cout) {
-  const int tiles = (Cout + 255) / 256;
+  const int tiles = (Cout + 127) / 128;
   int bn = (Cout + tiles - 1) / tiles;
-  bn = (bn + 15) & ~15;
-  if (bn < 16) bn = 16;
+  bn = (bn + 31) & ~31;
+  if (bn < 32) bn = 32;
   return bn;
 }
 
@@ -621,7 +351,7 @@ void conv_tc_prepare(ConvW& cw, DevBlob& blob, cudaStream_t st) {
   const size_t n = (size_t)cw.tc_npad * cw.tc_kpad;
   uint16_t* wh = (uint16_t*)blob.alloc_f((n + 1) / 2 + 4);
   uint16_t* wm = (uint16_t*)blob.alloc_f((n + 1) / 2 + 4);
-  int blocks = (int)((n + 255) / 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = (int)((n + 255) / 256); if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
   split_weights_kernel<<<blocks, 256, 0, st>>>(cw.w, K, cw.Cout, cw.ldw, wh, wm, cw.tc_kpad, cw.tc_npad);
   CUDA_OK(cudaGetLastError());
   cw.wh = wh; cw.wm = wm;
@@ -633,7 +363,7 @@ void conv_tc_prepare(ConvW& cw, DevBlob& blob, cudaStream_t st) {
     const size_t np = (size_t)cw.tc_npad * cw.ntaps * cp;
     uint16_t* whp = (uint16_t*)blob.alloc_f((np + 1) / 2 + 4);
     uint16_t* wmp = (uint16_t*)blob.alloc_f((np + 1) / 2 + 4);
-    int b2 = (int)((np + 255) / 256); if (b2 > 148 * 16) b2 = 148 * 16;
+    int b2 = (int)((np + 255) / 256); if (b2 > device_sm_count() * 16) b2 = device_sm_count() * 16;
     split_weights_padded_kernel<<<b2, 256, 0, st>>>(cw.w, cw.ntaps, cw.Cin, cp, cw.Cout, cw.ldw, whp, wmp, cw.tc_npad);
     CUDA_OK(cudaGetLastError());
     cw.whp = whp; cw.wmp = wmp; cw.tc_cp = cp;
@@ -648,7 +378,7 @@ void conv_tc_prepare(ConvW& cw, DevBlob& blob, cudaStream_t st) {
       const size_t n8 = (size_t)cw.tc_npad * kh * 64;
       uint16_t* w8h = (uint16_t*)blob.alloc_f((n8 + 1) / 2 + 4);
       uint16_t* w8m = (uint16_t*)blob.alloc_f((n8 + 1) / 2 + 4);
-      int b3 = (int)((n8 + 255) / 256); if (b3 > 148 * 16) b3 = 148 * 16;
+      int b3 = (int)((n8 + 255) / 256); if (b3 > device_sm_count() * 16) b3 = device_sm_count() * 16;
       split_weights_stem8_kernel<<<b3, 256, 0, st>>>(cw.w, kh, kw, cw.Cout, cw.ldw, w8h, w8m, cw.tc_npad);
       CUDA_OK(cudaGetLastError());
       cw.w8h = w8h; cw.w8m = w8m; cw.w8_kh = kh; cw.w8_kw = kw;
@@ -704,36 +434,25 @@ void launch_conv_tc(const ConvOp& op, cudaStream_t st) {
     if (op.tdx[t] > p.tmax_dx) p.tmax_dx = op.tdx[t];
   }
   p.sy = op.sy; p.sx = op.sx; p.pad = op.pad; p.Ho = op.Ho; p.Wo = op.Wo;
-  p.out = op.out.p; p.oH = op.out.H; p.oW = op.out.W; p.out_cs = op.out.cs; p.out_coff = op.out.coff; p.Cout = op.out.C;
-  p.out_planar = op.out.planar; p.oy_mul = op.oy_mul; p.oy_add = op.oy_add; p.ox_mul = op.ox_mul; p.ox_add = op.ox_add;
   p.in_scale = op.in_scale; p.in_shift = op.in_shift; p.in_relu = op.in_relu;
-  p.add0 = op.add0.p; p.add0_cs = op.add0.cs; p.add0_coff = op.add0.coff; p.add0_planar = op.add0.planar;
-  p.add1 = op.add1.p; p.add1_cs = op.add1.cs; p.add1_coff = op.add1.coff; p.add1_planar = op.add1.planar;
-  p.scale = op.scale; p.shift = op.shift; p.mul1 = op.mul1; p.act = op.act;
-  p.stat_max = op.stat_max; p.stat_sum = op.stat_sum; p.stat_idx = op.stat_idx; p.stat_ld = op.stat_ld;
+  fill_epi(p.e, op);
   MITB_CHECK(!op.stat_max || op.stat_ld == 2 * (op.tc_npad / op.tc_bn), "tc conv: stat_ld must equal conv_stat_blocks(op)");
-  p.M = op.in.N * op.Ho * op.Wo; p.K = op.ntaps * op.in.C; p.BN = op.tc_bn;
-  MITB_CHECK(p.BN >= 16 && p.BN <= 256 && p.BN % 16 == 0, "tc conv: bad BN %d", p.BN);
+  p.M = op.in.N * op.Ho * op.Wo; p.K = op.ntaps * op.in.C;
+  const int BN = op.tc_bn;
+  MITB_CHECK(BN >= 32 && BN <= 128 && BN % 32 == 0, "tc conv: bad BN %d", BN);
   MITB_CHECK(p.in_planar || p.Cin % 4 == 0, "tc conv: Cin must be a multiple of 4");
   MITB_CHECK((size_t)op.in.pixels() * op.in.cs < (size_t)1 << 31, "tc conv: input tensor too large for 32-bit element offsets");
-  int cols = 32; while (cols < p.BN) cols <<= 1;
-  p.tmem_cols = 2 * cols;                                  // double-buffered accumulator
-  const size_t stage_bytes = 2 * (size_t)TC_BM * 128 + 2 * (size_t)p.BN * 128;
-  const size_t epi_bytes = (size_t)TC_AWARPS * 32 * 20 * sizeof(float);
-  int stages = (int)((227 * 1024 - 1024 - 256 - epi_bytes) / stage_bytes); if (stages > 4) stages = 4;
-  MITB_CHECK(stages >= 2, "tc conv: tile does not fit shared memory");
-  p.stages = stages;
-  const size_t smem = stages * stage_bytes + (2 * stages + 6) * 8 + epi_bytes + 1024;
+  const size_t stage_bytes = 2 * (size_t)TC_BM * 128 + 2 * (size_t)BN * 128;
+  const size_t smem = 2 * stage_bytes + 2 * 8 + 1024;
   const int num_sms = device_sm_count();
   static PerDeviceOnce tc_attr;
   if (tc_attr.first()) {
-    CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<ACT_NONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<ACT_RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<ACT_GELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<ACT_SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<-1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   }
-  const int mt = (p.M + TC_BM - 1) / TC_BM, nt = p.npad / p.BN;
+  const int mt = (p.M + TC_BM - 1) / TC_BM, nt = p.npad / BN;
   // split-K for layers whose tile count cannot fill the SMs (deep, spatially tiny layers of the DBNet decoder)
   const int tiles = mt * nt, nkb = p.kpad / TC_BK;
   int splits = 1;
@@ -742,26 +461,25 @@ void launch_conv_tc(const ConvOp& op, cudaStream_t st) {
     if (splits > nkb / 4) splits = nkb / 4;
     if (splits < 1) splits = 1;
   }
-  p.splits = splits; p.partial = nullptr;
+  p.splits = splits;
   if (splits > 1) {
     const size_t need = (size_t)splits * p.M * p.npad * sizeof(float);
     static DeviceScratch g_partial;                                           // split-K partial sums
-    p.partial = static_cast<float*>(g_partial.get(need));
+    p.e.partial = static_cast<float*>(g_partial.get(need)); p.e.npad = p.npad;
   }
   const int total_tiles = tiles * splits;
   const int grid = total_tiles < num_sms ? total_tiles : num_sms;      // persistent: one CTA per SM
-  switch (splits > 1 || op.stat_max ? ACT_NONE : p.act) {
-    case ACT_NONE: conv_tc_kernel<ACT_NONE><<<grid, TC_THREADS, smem, st>>>(p); break;
-    case ACT_RELU: conv_tc_kernel<ACT_RELU><<<grid, TC_THREADS, smem, st>>>(p); break;
-    case ACT_GELU: conv_tc_kernel<ACT_GELU><<<grid, TC_THREADS, smem, st>>>(p); break;
-    case ACT_SILU: conv_tc_kernel<ACT_SILU><<<grid, TC_THREADS, smem, st>>>(p); break;
-    default: conv_tc_kernel<-1><<<grid, TC_THREADS, smem, st>>>(p); break;
+  switch (BN) {
+    case 32: conv_tc_kernel<32><<<grid, TC_THREADS, smem, st>>>(p); break;
+    case 64: conv_tc_kernel<64><<<grid, TC_THREADS, smem, st>>>(p); break;
+    case 96: conv_tc_kernel<96><<<grid, TC_THREADS, smem, st>>>(p); break;
+    default: conv_tc_kernel<128><<<grid, TC_THREADS, smem, st>>>(p); break;
   }
   count_launch();
   if (splits > 1) {
-    const long total = (long)p.M * ((p.Cout + 3) / 4);
-    int blocks = (int)((total + 255) / 256); if (blocks > 148 * 8) blocks = 148 * 8;
-    splitk_reduce_kernel<<<blocks, 256, 0, st>>>(p);
+    const long total = (long)p.M * ((op.out.C + 3) / 4);
+    int blocks = (int)((total + 255) / 256); if (blocks > num_sms * 8) blocks = num_sms * 8;
+    splitk_reduce_kernel<<<blocks, 256, 0, st>>>(p.e, splits);
     count_launch();
   }
   CUDA_OK(cudaGetLastError());

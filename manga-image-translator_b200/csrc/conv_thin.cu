@@ -3,9 +3,8 @@
 // value would be re-fetched 49 times from L2 (39 GB of gather traffic).  Here a CTA stages the input tile with its 3-pixel
 // halo in shared memory ONCE per 8-channel slab (planar [c][y][x] layout, reflect/zero padding resolved while staging)
 // and each thread produces 4 horizontally adjacent pixels x Cout channels from registers:
-//   per (channel, tap row): 3 LDS.128 of inputs + 7 broadcast LDS.128 of weights feed 56 FFMA2 (packed fp32x2: two output
-//   channels per instruction, the input value broadcast to both lanes)  ->  FMA-pipe bound (at 33 TF/s the scalar-FFMA version sat at
-//   ~0.9 of the 3-register FFMA issue rate).
+//   per (channel, tap row): 3 LDS.128 of inputs + 7 broadcast LDS.128 of weights feed 56 fp32 pair FMAs (two output channels
+//   per pair, the input value broadcast to both)  ->  FMA-pipe bound.
 #include "mitb_internal.h"
 
 namespace mitb {
@@ -74,7 +73,7 @@ __global__ void __launch_bounds__(256, 2) conv7_thin_kernel(const ThinParams p) 
       return;
     }
   }
-  float2 acc[4][2];                                      // [pixel][output-channel pair]: the taps run on the packed fp32x2 pipe
+  float2 acc[4][2];                                      // [pixel][output-channel pair]
 #pragma unroll
   for (int i = 0; i < 4; ++i) { acc[i][0] = make_float2(0.f, 0.f); acc[i][1] = make_float2(0.f, 0.f); }
 
@@ -120,9 +119,9 @@ __global__ void __launch_bounds__(256, 2) conv7_thin_kernel(const ThinParams p) 
           const float2 w01 = make_float2(wv.x, wv.y), w23 = make_float2(wv.z, wv.w);
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
-            const float x = in[1 + i + dx];                 // scalar operand broadcast to both lanes (SASS: FFMA2 ... R.F32)
-            acc[i][0] = __ffma2_rn(make_float2(x, x), w01, acc[i][0]);
-            acc[i][1] = __ffma2_rn(make_float2(x, x), w23, acc[i][1]);
+            const float x = in[1 + i + dx];                 // scalar operand broadcast to both channels
+            acc[i][0] = ffma2(make_float2(x, x), w01, acc[i][0]);
+            acc[i][1] = ffma2(make_float2(x, x), w23, acc[i][1]);
           }
         }
       }

@@ -1,25 +1,22 @@
-// TMA-fed tcgen05 implicit-GEMM convolution for sm_100a (stride 1 or 2, Cin a multiple of 8; the main conv path).
+// TMA-fed wgmma implicit-GEMM convolution for sm_90a (stride 1 or 2, Cin a multiple of 8; the main conv path).
 //
-// conv_tc.cu gathers the fp32 activation tile with producer warps and splits it into bf16 hi/mid inside the main loop.
-// Measured on B200 that loop is bound by the producers' own instruction stream (~650 dependent instructions per K block per
-// warp, 2 producer warps per scheduler): with loads, conversion, weight TMA and even the MMAs removed the kernel skeleton
-// still needs ~2600 cycles per K block against a tensor floor of 768 (profiles/r01_tc_skeleton_experiments.txt), and a 3x3
-// conv repeats the conversion of every input element 9 times (once per tap) per N tile.
-//
-// Here the conversion happens ONCE per input element in a separate memory-bound pass (split_pad_kernel: fp32 view ->
-// dense bf16 hi / mid NHWC tensors, optional BN+ReLU prologue, reflect halo materialised, planar inputs transposed), and the
-// GEMM main loop has no producer warps at all:
-//   warp 9   one thread: per K block (= 64 channels of one tap) four TMA loads - the activation box {64 ch, bw, bh} of the
-//            hi and mid tensors at the tap-shifted pixel coordinates (zero padding = TMA out-of-bounds fill) and the
-//            weight boxes {64 k, BN} - all landing in the UMMA K-major SWIZZLE_128B layout, completing on the stage's
-//            "full" mbarrier (expect_tx);
-//   warp 8   one thread: 12 tcgen05.mma per K block (bf16x3: Ah*Bh + Ah*Bm + Am*Bh), tcgen05.commit -> "empty" barrier;
-//   warps 0-7 epilogue: TMEM -> registers -> (+add0)*scale+shift -> act -> *mul1 -> +add1 -> coalesced fp32 stores through a
-//            shared-memory transpose; double-buffered accumulator, so tile i drains while tile i+1 is multiplied.
+// conv_tc.cu gathers the fp32 activation tile with the MMA warps and splits it into bf16 hi/mid inside the main loop, and a
+// 3x3 conv repeats the conversion of every input element 9 times (once per tap) per N tile.  Here the conversion happens ONCE
+// per input element in a separate memory-bound pass (split_pad_kernel: fp32 view -> dense bf16 hi / mid NHWC tensors, optional
+// BN+ReLU prologue, reflect halo materialised, planar inputs transposed), and the GEMM main loop only moves operands by TMA:
+//   warp 8      producer: per K block (= 64 channels of one tap) four TMA loads - the activation box {64 ch, bw, bh} of the
+//               hi and mid tensors at the tap-shifted pixel coordinates (zero padding = TMA out-of-bounds fill) and the
+//               weight boxes {64 k, BN} - all landing in the K-major SWIZZLE_128B layout, completing on the stage's "full"
+//               mbarrier (expect_tx); a ring of 3..6 stages;
+//   warps 0-7   two consumer warpgroups, 64 rows of the 128-row tile each: 12 wgmma per K block (bf16x3: Ah*Bh + Ah*Bm + Am*Bh,
+//               fp32 accumulators in registers), the stage is released on its "empty" mbarrier once the wgmma that read it
+//               retired (one K block of wgmma stays in flight); then the epilogue straight from the accumulator registers
+//               ((+add0)*scale+shift -> act -> *mul1 -> +add1 -> fp32 stores and / or split operands, tc_common.cuh) while the
+//               producer already streams the next tile's operands.
 // Operand fusion (ConvOp::in_sv / out_sv / seg2): a producer's epilogue can store its result directly as the consumer's bf16
 // hi/mid operand tensor (SplitView, optionally with a reflect halo and the consumer's BN+ReLU prologue applied), so the split
 // pass disappears; and a second K segment with its own tensor maps lets two convolutions of different inputs accumulate into one
-// TMEM accumulator (FFC: conv1x1(U) + conv3x3_{l->g}(x_l) -> BN_g -> ReLU -> +residual in ONE launch).
+// accumulator (FFC: conv1x1(U) + conv3x3_{l->g}(x_l) -> BN_g -> ReLU -> +residual in ONE launch).
 // An output tile is a bh x bw pixel patch of one image (bw*bh = 128, bw a power of two) so that a tap is a rectangular TMA
 // box; 1x1 convs use the flattened [pixels][C] matrix (bw = 128, bh = 1).  Persistent CTAs, one per SM.
 #include <cuda.h>
@@ -27,7 +24,6 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <cuda_bf16.h>
-#include <type_traits>
 #include "mitb_internal.h"
 
 namespace mitb {
@@ -35,10 +31,10 @@ namespace mitb {
 namespace {
 
 constexpr int TC_BM = 128, TC_BK = 64;
-constexpr int TM_EWARPS = 12;               // 3 epilogue warps per scheduler: short-K layers are bound by epilogue LATENCY (2 warps left the schedulers ~70 % idle)
-constexpr int TM_EPARTS = TM_EWARPS / 4;     // column parts per TMEM lane quarter
-constexpr int TM_MMAWARP = TM_EWARPS, TM_TMAWARP = TM_EWARPS + 1;
-constexpr int TM_THREADS = (TM_EWARPS + 2) * 32;
+constexpr int TM_CWARPS = 8;                         // two consumer warpgroups
+constexpr int TM_THREADS = TM_CWARPS * 32 + 32;      // + the producer warp
+
+#include "tc_common.cuh"
 
 struct SegParams {                                             // one K segment = one input tensor
   CUtensorMap ta_hi, ta_mid;                                  // activations: 4-D (C, Wp, Hp, N) bf16, box {64, bw, bh, 1}
@@ -50,63 +46,11 @@ struct TmaParams {
   int N, Ho, Wo, M, lin;                                      // lin: tile = 128 consecutive rows of the flattened [M][C] matrix
   int sy, sx;                                                 // conv stride (TMA element strides of the activation box)
   int bw_log2, tiles_x, tiles_y;
-  int npad, BN, stages, tmem_cols;
-  float* out; int oH, oW, out_cs, out_coff, Cout, out_planar, oy_mul, oy_add, ox_mul, ox_add;
-  const float* add0; int add0_cs, add0_coff, add0_planar;
-  const float* add1; int add1_cs, add1_coff, add1_planar;
-  const float* scale; const float* shift; const float* mul1; int act;
-  float* stat_max; float* stat_sum; int* stat_idx; int stat_ld;
-  // split output (ConvOp::out_sv): bf16 hi / mid at [((n*os_Hp + y + os_pt)*os_Wp + x + os_pl)*os_pitch + os_coff + c] (null: none)
-  uint16_t* os_hi; uint16_t* os_mid; int os_pitch, os_coff, os_Hp, os_Wp, os_pt, os_pl;
-  const float* os_scale; const float* os_shift; int os_relu;  // consumer prologue applied before splitting
-  int fast;                                                   // NHWC, 16-byte aligned rows / constants, Cout % 4 == 0: the packed epilogue
+  int npad, stages;
   const uint8_t* tile_need;                                   // per 128-row M tile: 0 = skip (ConvOp::need_px reduced over the tile), null: all
+  EpiParams e;
 };
 
-#include "tc_common.cuh"
-
-__device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const CUtensorMap* map, uint32_t bar, int c, int x, int y, int n) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(smem_dst), "l"(map), "r"(bar), "r"(c), "r"(x), "r"(y), "r"(n) : "memory");
-}
-
-// One K block of the bf16x3 product: for each of the four 16-wide k steps Ah*Bh, Ah*Bm, Am*Bh, then tcgen05.commit on the
-// stage's "empty" barrier - issued by one elected lane of a converged warp (operands stay in uniform registers).
-__device__ __forceinline__ void umma_kblock_x3(uint32_t tmem_d, uint64_t dah, uint64_t dam, uint64_t dbh, uint64_t dbm, uint32_t idesc,
-                                               uint32_t acc_first, uint32_t empty_bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred pe, pa, pt;\n"
-      ".reg .b64 ah, am, bh, bm;\n"
-      "elect.sync _|pe, 0xffffffff;\n"
-      "setp.ne.b32 pa, %6, 0;\n"
-      "setp.eq.u32 pt, %5, %5;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %3, %5, pa;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %4, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %2, %3, %5, pt;\n"
-      "add.s64 ah, %1, 2;\n add.s64 am, %2, 2;\n add.s64 bh, %3, 2;\n add.s64 bm, %4, 2;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], ah, bh, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], ah, bm, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], am, bh, %5, pt;\n"
-      "add.s64 ah, %1, 4;\n add.s64 am, %2, 4;\n add.s64 bh, %3, 4;\n add.s64 bm, %4, 4;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], ah, bh, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], ah, bm, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], am, bh, %5, pt;\n"
-      "add.s64 ah, %1, 6;\n add.s64 am, %2, 6;\n add.s64 bh, %3, 6;\n add.s64 bm, %4, 6;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], ah, bh, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], ah, bm, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], am, bh, %5, pt;\n"
-      "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%7];\n"
-      "}\n" ::"r"(tmem_d), "l"(dah), "l"(dam), "l"(dbh), "l"(dbm), "r"(idesc), "r"(acc_first), "r"(empty_bar) : "memory");
-}
-__device__ __forceinline__ void umma_commit_elect(uint32_t bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred pe;\n"
-      "elect.sync _|pe, 0xffffffff;\n"
-      "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-      "}\n" ::"r"(bar) : "memory");
-}
 // expect_tx + the four operand boxes of one K block, issued by one elected lane of a converged warp
 __device__ __forceinline__ void tma_kblock(uint32_t bar, uint32_t bytes, uint32_t a_hi, uint32_t a_mid, uint32_t b_hi, uint32_t b_mid,
                                            const CUtensorMap* ta_hi, const CUtensorMap* ta_mid, const CUtensorMap* tb_hi,
@@ -124,458 +68,88 @@ __device__ __forceinline__ void tma_kblock(uint32_t bar, uint32_t bytes, uint32_
       "r"(c), "r"(x), "r"(y), "r"(n), "r"(k), "r"(n0) : "memory");
 }
 
-// ---- CTA-pair (cta_group::2) variants: one 256 x BN tile per pair of SMs, each CTA stages its own 128 rows of A and HALF of B
-__device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {
-  uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank)); return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
-  // default semantics (release at CTA scope), like CUTLASS' ClusterBarrier::arrive(cta_id): an explicit .release.cluster costs a
-  // cluster-scope membar per arrive (ncu: membar stalls, 1.5x slower K loop) and orders nothing we need - the accumulator reads
-  // are ordered by tcgen05.fence::before_thread_sync, the operand bytes by the mbarrier's transaction count
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void umma_kblock_x3_pair(uint32_t tmem_d, uint64_t dah, uint64_t dam, uint64_t dbh, uint64_t dbm, uint32_t idesc,
-                                                    uint32_t acc_first, uint32_t empty_bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred pe, pa, pt;\n"
-      ".reg .b64 ah, am, bh, bm;\n"
-      ".reg .b16 msk;\n"
-      "mov.b16 msk, 3;\n"
-      "elect.sync _|pe, 0xffffffff;\n"
-      "setp.ne.b32 pa, %6, 0;\n"
-      "setp.eq.u32 pt, %5, %5;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %3, %5, pa;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %4, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], %2, %3, %5, pt;\n"
-      "add.s64 ah, %1, 2;\n add.s64 am, %2, 2;\n add.s64 bh, %3, 2;\n add.s64 bm, %4, 2;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], ah, bh, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], ah, bm, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], am, bh, %5, pt;\n"
-      "add.s64 ah, %1, 4;\n add.s64 am, %2, 4;\n add.s64 bh, %3, 4;\n add.s64 bm, %4, 4;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], ah, bh, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], ah, bm, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], am, bh, %5, pt;\n"
-      "add.s64 ah, %1, 6;\n add.s64 am, %2, 6;\n add.s64 bh, %3, 6;\n add.s64 bm, %4, 6;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], ah, bh, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], ah, bm, %5, pt;\n"
-      "@pe tcgen05.mma.cta_group::2.kind::f16 [%0], am, bh, %5, pt;\n"
-      "@pe tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%7], msk;\n"
-      "}\n" ::"r"(tmem_d), "l"(dah), "l"(dam), "l"(dbh), "l"(dbm), "r"(idesc), "r"(acc_first), "r"(empty_bar) : "memory");
-}
-__device__ __forceinline__ void umma_commit_elect_pair(uint32_t bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred pe;\n"
-      ".reg .b16 msk;\n"
-      "mov.b16 msk, 3;\n"
-      "elect.sync _|pe, 0xffffffff;\n"
-      "@pe tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], msk;\n"
-      "}\n" ::"r"(bar) : "memory");
-}
-// expect_tx on the LEADER's full barrier (cluster address) + this CTA's four operand boxes completing on it
-__device__ __forceinline__ void tma_kblock_pair(uint32_t lead_bar, uint32_t bytes, uint32_t a_hi, uint32_t a_mid, uint32_t b_hi, uint32_t b_mid,
-                                                const CUtensorMap* ta_hi, const CUtensorMap* ta_mid, const CUtensorMap* tb_hi,
-                                                const CUtensorMap* tb_mid, int c, int x, int y, int n, int k, int n0) {
-  asm volatile(
-      "{\n"
-      ".reg .pred pe;\n"
-      "elect.sync _|pe, 0xffffffff;\n"
-      "@pe mbarrier.arrive.expect_tx.shared::cluster.b64 _, [%0], %1;\n"
-      "@pe cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%2], [%6, {%10, %11, %12, %13}], [%0];\n"
-      "@pe cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%3], [%7, {%10, %11, %12, %13}], [%0];\n"
-      "@pe cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%4], [%8, {%14, %15}], [%0];\n"
-      "@pe cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%5], [%9, {%14, %15}], [%0];\n"
-      "}\n" ::"r"(lead_bar), "r"(bytes), "r"(a_hi), "r"(a_mid), "r"(b_hi), "r"(b_mid), "l"(ta_hi), "l"(ta_mid), "l"(tb_hi), "l"(tb_mid),
-      "r"(c), "r"(x), "r"(y), "r"(n), "r"(k), "r"(n0) : "memory");
-}
-
-// CG = 1: one CTA per 128 x BN tile.  CG = 2: clusters of two CTAs (one SM pair) share a 256 x BN tile through tcgen05 cta_group::2:
-// CTA r owns rows [128 r, 128 r + 128) (its own activation boxes, its own TMEM accumulator, its own epilogue) and stages only rows
-// [r BN/2, (r+1) BN/2) of the weight tile, so the weight bytes each SM pulls from L2 halve - these GEMMs are bound by the ~42 B/clk
-// an SM gets from L2 (hi + mid operands), not by the tensor pipe.  The leader (rank 0) issues every MMA; full barriers live in the
-// leader and collect both CTAs' TMA bytes, tcgen05.commit multicasts the stage-free / accumulator-ready arrivals to both CTAs.
-template <int ACT, int CG>
+template <int ACT, int BN>
 __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_constant__ TmaParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int BN = p.BN, S = p.stages;
-  const uint32_t a_bytes = TC_BM * 128, b_bytes = (uint32_t)(BN / CG) * 128;         // CG = 2: half of the weight tile per CTA
-  const uint32_t stage_bytes = 2 * a_bytes + 2 * b_bytes;
-  const uint32_t crank = CG == 2 ? cluster_rank() : 0u;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);   // full[S], empty[S], tfull[2], tempty[2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 4);
-  float* estage = reinterpret_cast<float*>(bars + 2 * S + 6);          // [TM_EWARPS][32 rows][20 floats] epilogue transpose buffer
+  const int S = p.stages;
+  constexpr uint32_t a_bytes = TC_BM * 128, b_bytes = (uint32_t)BN * 128;
+  constexpr uint32_t stage_bytes = 2 * a_bytes + 2 * b_bytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);   // full[S], empty[S]
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar_base = smem_u32(bars);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (2 * S + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (2 * S + 2 + b); };
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // warp-uniform to the compiler: wgmma stays unserialized
   const int nkb = p.nkb;
   const int bw = 1 << p.bw_log2, bh = TC_BM >> p.bw_log2;
   const int mt = p.N * p.tiles_y * p.tiles_x, nt = p.npad / BN;
-  const int total_tiles = ((mt + CG - 1) / CG) * nt;                 // CG = 2: pair tiles (two consecutive 128-row tiles)
-  const int tile_first = CG == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_step = CG == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const uint32_t acc_stride = (uint32_t)(p.tmem_cols >> 1);
+  const int total_tiles = mt * nt;
 
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), CG); mbar_init(empty_bar(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tfull_bar(b), 1); mbar_init(tempty_bar(b), CG * TM_EWARPS); }
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TM_CWARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == TM_MMAWARP) tmem_alloc(smem_u32(tmem_slot), (uint32_t)p.tmem_cols);
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();             // peers must see initialised barriers before any remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
-  // tile t -> (image, patch origin, N tile); N fastest so CTAs running together share the activation boxes in L2.
-  // A pair's second CTA may get an m-tile past the end (odd tile count): nimg == N there, TMA fills zeros, stores are masked.
+  // tile t -> (image, patch origin, N tile); N fastest so CTAs running together share the activation boxes in L2
   auto decode = [&](int t, int& nimg, int& oy0, int& ox0, int& n0) {
-    const int mpair = t / nt; n0 = (t - mpair * nt) * BN;
-    const int mtile = CG == 2 ? 2 * mpair + (int)crank : mpair;
+    const int mtile = t / nt; n0 = (t - mtile * nt) * BN;
     const int per_img = p.tiles_y * p.tiles_x;
     nimg = mtile / per_img; const int r = mtile - nimg * per_img;
     const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
     oy0 = ty * bh; ox0 = tx * bw;
   };
+  // output sparsity: every role walks the same tile sequence and skips the same tiles
+  auto needed = [&](int t) -> bool { return !p.tile_need || p.tile_need[t / nt] != 0; };
 
-  // output sparsity: every role walks the same tile sequence and skips the same tiles (a pair tile is needed if either half is)
-  auto needed = [&](int t) -> bool {
-    if (!p.tile_need) return true;
-    const int mpair = t / nt;
-    if (CG == 2) return (p.tile_need[2 * mpair] | (2 * mpair + 1 < mt ? p.tile_need[2 * mpair + 1] : (uint8_t)0)) != 0;
-    return p.tile_need[mpair] != 0;
-  };
-
-  if (warp < TM_EWARPS) {
-    // =========================== epilogue: warp w drains TMEM lane quarter (w & 3), column half (w >> 2) ===========================
-    const int q = warp & 3, epart = warp >> 2;       // TMEM lane quarter (must equal warp % 4), column part
+  if (warp < TM_CWARPS) {
+    // =========================== consumers: wgmma main loop + epilogue ===========================
+    const int wg = warp >> 2;
     const int HoWo = p.Ho * p.Wo;
-    const int nchunks = BN / 16, h0 = (nchunks + 1) / 2;
-    // the row-stat layout has two column halves per N tile (shared with conv_tc.cu): parts 0 / 1 take them, part 2 idles there
-    const int ehalf = epart;
-    const int cb_lo = p.stat_max ? (epart == 0 ? 0 : epart == 1 ? h0 : nchunks) * 16 : (nchunks * epart / TM_EPARTS) * 16;
-    const int cb_hi = p.stat_max ? (epart == 0 ? h0 : nchunks) * 16 : (nchunks * (epart + 1) / TM_EPARTS) * 16;
-    // row r of the tile -> output pixel (linear index into the Ho x Wo grid of image nimg), -1 when outside
-    auto row_pixel = [&](int r, int nimg_t, int oy0, int ox0, int& nimg, int& oy, int& ox) -> bool {
-      if (p.lin) {
-        const int m = ox0 + r;
-        if (m >= p.M || nimg_t >= p.N) return false;
-        nimg = m / HoWo; const int pp = m - nimg * HoWo;
-        oy = pp / p.Wo; ox = pp - oy * p.Wo;
-        return true;
-      }
-      nimg = nimg_t; oy = oy0 + (r >> p.bw_log2); ox = ox0 + (r & (bw - 1));
-      return oy < p.Ho && ox < p.Wo && nimg < p.N;
-    };
-    int lt = 0;
-    const uint32_t tempty_lead0 = CG == 2 ? mapa_rank(tempty_bar(0), 0) : tempty_bar(0);   // the MMA issuer (leader) owns "accumulator drained"
-    for (int t = tile_first; t < total_tiles; t += tile_step) {
+    int s = 0; uint32_t ph = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       if (!needed(t)) continue;
       int nimg_t, oy0, ox0, n0;
       decode(t, nimg_t, oy0, ox0, n0);
-      const int buf = lt & 1;
-      mbar_wait(tfull_bar(buf), (lt >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr_row = tmem_base + (uint32_t)buf * acc_stride + ((uint32_t)(q * 32) << 16);
-      if (p.stat_max) {
-        // vocabulary head: online (max, first argmax, sum exp) over this thread's columns of its row (model_48px_ctc.py:460-461)
-        int nimg, oy, ox;
-        const bool row_ok = row_pixel(q * 32 + lane, nimg_t, oy0, ox0, nimg, oy, ox);
-        float bm = -INFINITY, bs = 0.f; int bi = 0x7fffffff;
-#pragma unroll 1
-        for (int cb = cb_lo; cb < cb_hi; cb += 16) {
-          uint32_t raw[16];
-          tmem_ld16(taddr_row + (uint32_t)cb, raw);
-          tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const int c = n0 + cb + e;
-            if (c < p.Cout) {
-              const float x = __uint_as_float(raw[e]) + (p.shift ? __ldg(p.shift + c) : 0.f);
-              if (x > bm) { bs = bs * expf(bm - x) + 1.f; bm = x; bi = c; }
-              else bs += expf(x - bm);
-            }
-          }
-        }
-        if (row_ok && epart < 2) {
-          const size_t m = ((size_t)nimg * p.Ho + oy) * p.Wo + ox;
-          const size_t o = m * p.stat_ld + (n0 / BN) * 2 + ehalf;
-          p.stat_max[o] = bm; p.stat_sum[o] = bs; p.stat_idx[o] = bi;
-        }
-      } else if (p.fast) {
-        // ---- the common case (NHWC output, every per-channel constant and row 16-byte aligned, Cout % 4 == 0), written for
-        // instruction count: short-K layers (ConvNeXt fc1, the spectral 1x1 convs, the decoders) are bound by the epilogue's issue
-        // slots, not by the tensor pipe.  Arithmetic on the packed fp32x2 pipe, per-channel constants as one 16-byte load each,
-        // no per-element bounds checks, and the TMEM load of the next chunk in flight while this one is processed.  The 16-column
-        // chunks of a tile rotate over the TM_EPARTS warps of a lane quarter from tile to tile, so that chunk counts that do
-        // not divide by TM_EPARTS (BN = 128: 3 + 3 + 2) balance over consecutive tiles (the accumulator is double buffered).
-        const uint32_t st_w = smem_u32(estage + (size_t)warp * 32 * 20) + (uint32_t)lane * 80u;              // this lane's row of the staging tile
-        const int sub = lane & 3, rsel = lane >> 2;              // this thread: columns 4*sub..+3 of rows rsel + 8j
-        const uint32_t st_r = smem_u32(estage + (size_t)warp * 32 * 20) + (uint32_t)rsel * 80u + (uint32_t)sub * 16u;
-        // element offsets of this thread's four rows in the output / split output / residual tensors (host checked: < 2^31 elements)
-        uint32_t eo[4], so[4], ao[4], rmask = 0;
-        const float* addp = p.add0 ? p.add0 + p.add0_coff : p.add1 ? p.add1 + p.add1_coff : nullptr;
-        const int add_cs = p.add0 ? p.add0_cs : p.add1_cs;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          int nimg, oy, ox;
-          eo[j] = 0; so[j] = 0; ao[j] = 0;
-          if (row_pixel(q * 32 + rsel + 8 * j, nimg_t, oy0, ox0, nimg, oy, ox)) {
-            const uint32_t opix = (uint32_t)((nimg * p.oH + oy * p.oy_mul + p.oy_add) * p.oW + ox * p.ox_mul + p.ox_add);
-            eo[j] = opix * (uint32_t)p.out_cs + (uint32_t)p.out_coff;
-            ao[j] = opix * (uint32_t)add_cs;
-            so[j] = (uint32_t)((nimg * p.os_Hp + oy + p.os_pt) * p.os_Wp + ox + p.os_pl) * (uint32_t)p.os_pitch + (uint32_t)p.os_coff;
-            rmask |= 1u << j;
-          }
-        }
-        const bool extra = p.add0 || p.add1 || p.mul1;           // residual / layer-scale operands: only long-K layers have them
-        int nch = (p.Cout - n0 + 15) >> 4; if (nch > nchunks) nch = nchunks;      // chunks wholly past Cout are never touched
-        int c = (epart + TM_EPARTS - lt % TM_EPARTS) % TM_EPARTS;
-        uint32_t raw[16];
-        if (c < nch) tmem_ld16(taddr_row + (uint32_t)(c * 16), raw);
-#pragma unroll 1
-        for (; c < nch; c += TM_EPARTS) {
-          const int cq = n0 + c * 16 + 4 * sub;
-          const bool colok = cq < p.Cout;                       // Cout % 4 == 0: a thread's four columns are in or out together
-          float4 A[4];                                           // residual / branch-sum rows (at most one of add0 / add1 on this path)
-          if (addp) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              A[j] = (colok && ((rmask >> j) & 1u)) ? *reinterpret_cast<const float4*>(addp + (ao[j] + (uint32_t)cq)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-          float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (colok) {
-            if (p.scale) sc = __ldg(reinterpret_cast<const float4*>(p.scale + cq));
-            if (p.shift) sh = __ldg(reinterpret_cast<const float4*>(p.shift + cq));
-          }
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 4; ++i) sts128(st_w + 16u * i, raw[4 * i], raw[4 * i + 1], raw[4 * i + 2], raw[4 * i + 3]);
-          __syncwarp();
-          if (c + TM_EPARTS < nch) tmem_ld16(taddr_row + (uint32_t)((c + TM_EPARTS) * 16), raw);      // next chunk: latency hidden behind the math
-          if (colok) {
-            auto body = [&](auto extra_tag) {
-              constexpr bool EXTRA = decltype(extra_tag)::value;
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                if (!((rmask >> j) & 1u)) continue;
-                const float4 a = lds128(st_r + (uint32_t)j * 640u);
-                float2 v0 = make_float2(a.x, a.y), v1 = make_float2(a.z, a.w);
-                if (EXTRA && p.add0) { v0 = __fadd2_rn(v0, make_float2(A[j].x, A[j].y)); v1 = __fadd2_rn(v1, make_float2(A[j].z, A[j].w)); }
-                v0 = __ffma2_rn(v0, make_float2(sc.x, sc.y), make_float2(sh.x, sh.y));
-                v1 = __ffma2_rn(v1, make_float2(sc.z, sc.w), make_float2(sh.z, sh.w));
-                v0 = act_t2<ACT>(v0, p.act); v1 = act_t2<ACT>(v1, p.act);
-                if (EXTRA) {
-                  if (p.mul1) {                     // (layer scale: re-read per row from L1 - these long-K layers have the slack, the registers do not)
-                    const float4 mu = __ldg(reinterpret_cast<const float4*>(p.mul1 + cq));
-                    v0 = __fmul2_rn(v0, make_float2(mu.x, mu.y)); v1 = __fmul2_rn(v1, make_float2(mu.z, mu.w));
-                  }
-                  if (p.add1) { v0 = __fadd2_rn(v0, make_float2(A[j].x, A[j].y)); v1 = __fadd2_rn(v1, make_float2(A[j].z, A[j].w)); }
-                }
-                if (p.out) *reinterpret_cast<float4*>(p.out + (eo[j] + (uint32_t)cq)) = make_float4(v0.x, v0.y, v1.x, v1.y);
-                if (p.os_hi) {                       // producer -> consumer fusion: store the consumer's bf16 hi / mid operands directly
-                  if (p.os_scale) {
-                    const float4 osc = __ldg(reinterpret_cast<const float4*>(p.os_scale + cq)), osh = __ldg(reinterpret_cast<const float4*>(p.os_shift + cq));
-                    v0 = __ffma2_rn(v0, make_float2(osc.x, osc.y), make_float2(osh.x, osh.y));
-                    v1 = __ffma2_rn(v1, make_float2(osc.z, osc.w), make_float2(osh.z, osh.w));
-                    if (p.os_relu) { v0 = make_float2(fmaxf(v0.x, 0.f), fmaxf(v0.y, 0.f)); v1 = make_float2(fmaxf(v1.x, 0.f), fmaxf(v1.y, 0.f)); }
-                  }
-                  uint2 hh, mm;
-                  split4p(v0, v1, hh, mm);
-                  const uint32_t o = so[j] + (uint32_t)cq;
-                  *reinterpret_cast<uint2*>(p.os_hi + o) = hh;
-                  *reinterpret_cast<uint2*>(p.os_mid + o) = mm;
-                }
-              }
-            };
-            if (extra) body(std::true_type{}); else body(std::false_type{});
-          }
-          __syncwarp();
-        }
-      } else if (!p.out_planar && ((p.out_cs | p.out_coff) & 3) == 0 &&
-                 (!p.add0 || (!p.add0_planar && ((p.add0_cs | p.add0_coff) & 3) == 0)) &&
-                 (!p.add1 || (!p.add1_planar && ((p.add1_cs | p.add1_coff) & 3) == 0))) {
-        // ---- NHWC output: transpose 32x16 accumulator chunks through shared memory so that one warp instruction touches
-        // 8 rows x 64 contiguous bytes (residual reads and stores coalesced)
-        float* st = estage + (size_t)warp * 32 * 20;
-        const int sub = lane & 3, rsel = lane >> 2;              // this thread: columns 4*sub..+3 of rows rsel + 8j
-        size_t orow[4]; uint32_t srow[4]; uint32_t rmask = 0;    // srow: pixel index inside the (halo'd) split output tensor
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          int nimg, oy, ox;
-          orow[j] = 0; srow[j] = 0;
-          if (row_pixel(q * 32 + rsel + 8 * j, nimg_t, oy0, ox0, nimg, oy, ox)) {
-            orow[j] = ((size_t)nimg * p.oH + oy * p.oy_mul + p.oy_add) * p.oW + ox * p.ox_mul + p.ox_add;
-            srow[j] = (uint32_t)((nimg * p.os_Hp + oy + p.os_pt) * p.os_Wp + ox + p.os_pl);
-            rmask |= 1u << j;
-          }
-        }
-        // The residual / branch-sum operands of a chunk are requested right after its TMEM load is issued, so both latencies
-        // overlap (and the other two warps of the scheduler run meanwhile).
-        float4 pa0[4], pa1[4];
-        auto fetch_adds = [&](int cb, float4 (&A0)[4], float4 (&A1)[4]) {
-          const int cq = n0 + cb + 4 * sub;
-          const bool vec = cq + 3 < p.Cout;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            A0[j] = make_float4(0.f, 0.f, 0.f, 0.f); A1[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (!((rmask >> j) & 1u) || cq >= p.Cout) continue;
-            if (p.add0) {
-              const float* s0 = p.add0 + orow[j] * p.add0_cs + p.add0_coff + cq;
-              if (vec) A0[j] = *reinterpret_cast<const float4*>(s0);
-              else { A0[j].x = s0[0]; if (cq + 1 < p.Cout) A0[j].y = s0[1]; if (cq + 2 < p.Cout) A0[j].z = s0[2]; }
-            }
-            if (p.add1) {
-              const float* s1 = p.add1 + orow[j] * p.add1_cs + p.add1_coff + cq;
-              if (vec) A1[j] = *reinterpret_cast<const float4*>(s1);
-              else { A1[j].x = s1[0]; if (cq + 1 < p.Cout) A1[j].y = s1[1]; if (cq + 2 < p.Cout) A1[j].z = s1[2]; }
-            }
-          }
-        };
-#pragma unroll 1
-        for (int cb = cb_lo; cb < cb_hi; cb += 16) {
-          uint32_t raw[16];
-          tmem_ld16(taddr_row + (uint32_t)cb, raw);
-          if (p.add0 || p.add1) fetch_adds(cb, pa0, pa1);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            *reinterpret_cast<uint4*>(st + lane * 20 + 4 * i) = make_uint4(raw[4 * i], raw[4 * i + 1], raw[4 * i + 2], raw[4 * i + 3]);
-          __syncwarp();
-          const int cq = n0 + cb + 4 * sub;
-          if (cq < p.Cout) {
-            const bool full = cq + 3 < p.Cout;
-            float sc4[4] = {1.f, 1.f, 1.f, 1.f}, sh4[4] = {0.f, 0.f, 0.f, 0.f}, mu4[4] = {1.f, 1.f, 1.f, 1.f};
-            float os_sc4[4] = {1.f, 1.f, 1.f, 1.f}, os_sh4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-              if (cq + e < p.Cout) {
-                if (p.scale) sc4[e] = __ldg(p.scale + cq + e);
-                if (p.shift) sh4[e] = __ldg(p.shift + cq + e);
-                if (p.mul1) mu4[e] = __ldg(p.mul1 + cq + e);
-                if (p.os_scale) { os_sc4[e] = __ldg(p.os_scale + cq + e); os_sh4[e] = __ldg(p.os_shift + cq + e); }
-              }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              if (!((rmask >> j) & 1u)) continue;
-              const float4 a = *reinterpret_cast<const float4*>(st + (rsel + 8 * j) * 20 + 4 * sub);
-              float v4[4] = {a.x, a.y, a.z, a.w};
-              if (p.add0) { v4[0] += pa0[j].x; v4[1] += pa0[j].y; v4[2] += pa0[j].z; v4[3] += pa0[j].w; }
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float x = v4[e];
-                if (p.scale) x *= sc4[e];
-                x += sh4[e];
-                x = act_t<ACT>(x, p.act);
-                if (p.mul1) x *= mu4[e];
-                v4[e] = x;
-              }
-              if (p.add1) { v4[0] += pa1[j].x; v4[1] += pa1[j].y; v4[2] += pa1[j].z; v4[3] += pa1[j].w; }
-              if (p.out) {
-                if (full) *reinterpret_cast<float4*>(p.out + orow[j] * p.out_cs + p.out_coff + cq) = make_float4(v4[0], v4[1], v4[2], v4[3]);
-                else { for (int e = 0; e < 4; ++e) if (cq + e < p.Cout) p.out[orow[j] * p.out_cs + p.out_coff + cq + e] = v4[e]; }
-              }
-              if (p.os_hi) {                         // producer -> consumer fusion: store the consumer's bf16 hi / mid operands directly
-                if (p.os_scale) {
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    v4[e] = fmaf(v4[e], os_sc4[e], os_sh4[e]);
-                    if (p.os_relu) v4[e] = fmaxf(v4[e], 0.f);
-                  }
-                }
-                uint2 hh, mm;
-                split4(make_float4(v4[0], v4[1], v4[2], v4[3]), hh, mm);
-                const size_t so = (size_t)srow[j] * p.os_pitch + p.os_coff + cq;
-                *reinterpret_cast<uint2*>(p.os_hi + so) = hh;
-                *reinterpret_cast<uint2*>(p.os_mid + so) = mm;
-              }
-            }
-          }
-          __syncwarp();
-        }
-      } else {
-        // ---- planar (NCHW) or unaligned output: lane = pixel, so each channel's stores are contiguous across lanes
-        int nimg = 0, oy = 0, ox = 0;
-        const bool row_ok = row_pixel(q * 32 + lane, nimg_t, oy0, ox0, nimg, oy, ox);
-        const int py = oy * p.oy_mul + p.oy_add, px = ox * p.ox_mul + p.ox_add;
-        const size_t opix = ((size_t)nimg * p.oH + py) * p.oW + px;
-        const size_t oplane = (size_t)p.oH * p.oW, opl_pix = (size_t)py * p.oW + px;
-#pragma unroll 1
-        for (int cb = cb_lo; cb < cb_hi; cb += 16) {
-          uint32_t raw[16];
-          tmem_ld16(taddr_row + (uint32_t)cb, raw);
-          tmem_ld_wait();
-          if (!row_ok) continue;
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const int c = n0 + cb + e;
-            if (c >= p.Cout) break;
-            float x = __uint_as_float(raw[e]);
-            if (p.add0) x += p.add0_planar ? p.add0[((size_t)nimg * p.add0_cs + p.add0_coff + c) * oplane + opl_pix] : p.add0[opix * p.add0_cs + p.add0_coff + c];
-            if (p.scale) x *= __ldg(p.scale + c);
-            if (p.shift) x += __ldg(p.shift + c);
-            x = act_t<ACT>(x, p.act);
-            if (p.mul1) x *= __ldg(p.mul1 + c);
-            if (p.add1) x += p.add1_planar ? p.add1[((size_t)nimg * p.add1_cs + p.add1_coff + c) * oplane + opl_pix] : p.add1[opix * p.add1_cs + p.add1_coff + c];
-            if (p.out_planar) p.out[((size_t)nimg * p.out_cs + p.out_coff + c) * oplane + opl_pix] = x;
-            else p.out[opix * p.out_cs + p.out_coff + c] = x;
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {                                     // accumulator drained -> the MMA warp may overwrite it
-        if (CG == 2) mbar_arrive_cluster(tempty_lead0 + 8u * buf); else mbar_arrive(tempty_bar(buf));
-      }
-      ++lt;
-    }
-  } else if (warp == TM_MMAWARP) {
-    // =========================== MMA issuer ===========================
-    // The whole warp runs the (warp-uniform) loop and one elected lane issues: descriptors and barrier addresses then live in
-    // uniform registers and a K block costs ~40 SASS instructions.  With the loop inside `if (lane == 0)` the compiler
-    // moved every operand of every tcgen05.mma through R2UR/ELECT sequences: ~350 dependent instructions per K block on this
-    // single warp, i.e. ~1400 cycles against the 768-cycle tensor floor of a 128x128x64 bf16x3 block (ncu, r01).
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)((CG * TC_BM) >> 4) << 24);
-    int s = 0; uint32_t ph = 0; int lt = 0;
-    if (CG == 1 || crank == 0)
-    for (int t = tile_first; t < total_tiles; t += tile_step) {
-      if (!needed(t)) continue;
-      const int buf = lt & 1;
-      mbar_wait(tempty_bar(buf), ((lt >> 1) & 1) ^ 1);             // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)buf * acc_stride;
+      float acc[BN / 2];
+      int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(full_bar(s), ph);
-        tc_fence_after();
-        const uint32_t a_hi = smem_base + (uint32_t)s * stage_bytes, a_mid = a_hi + a_bytes;
-        const uint32_t b_hi = a_mid + a_bytes, b_mid = b_hi + b_bytes;
-        if (CG == 2)
-          umma_kblock_x3_pair(tmem_d, make_desc_sw128(a_hi), make_desc_sw128(a_mid), make_desc_sw128(b_hi), make_desc_sw128(b_mid), idesc,
-                              kb > 0 ? 1u : 0u, empty_bar(s));       // 12 pair MMAs + commit multicast -> frees the stage in both CTAs
-        else
-          umma_kblock_x3(tmem_d, make_desc_sw128(a_hi), make_desc_sw128(a_mid), make_desc_sw128(b_hi), make_desc_sw128(b_mid), idesc,
-                         kb > 0 ? 1u : 0u, empty_bar(s));            // 12 MMAs + commit -> frees the stage when they retire
+        const uint32_t a_hi = smem_base + (uint32_t)s * stage_bytes + (uint32_t)wg * (64u * 128u), a_mid = a_hi + a_bytes;
+        const uint32_t b_hi = smem_base + (uint32_t)s * stage_bytes + 2 * a_bytes, b_mid = b_hi + b_bytes;
+        fence_acc(acc);
+        wgmma_fence();
+        wgmma_kblock_x3<BN>(acc, make_desc_sw128(a_hi), make_desc_sw128(a_mid), make_desc_sw128(b_hi), make_desc_sw128(b_mid), kb == 0);
+        wgmma_commit();
+        wgmma_wait<1>();                                 // the previous K block's wgmma retired -> its stage is free
+        fence_acc(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+        prev = s;
         if (++s == S) { s = 0; ph ^= 1u; }
       }
-      if (CG == 2) umma_commit_elect_pair(tfull_bar(buf)); else umma_commit_elect(tfull_bar(buf));      // accumulator complete -> epilogue(s)
-      ++lt;
+      wgmma_wait<0>();
+      fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(prev));
+      epilogue_tile<ACT, BN>(p.e, acc, wg * 64 + (warp & 3) * 16 + (lane >> 2), n0, 0, [&](int r, int& nimg, int& oy, int& ox) -> bool {
+        if (p.lin) {
+          const int m = ox0 + r;
+          if (m >= p.M || nimg_t >= p.N) return false;
+          nimg = m / HoWo; const int pp = m - nimg * HoWo;
+          oy = pp / p.Wo; ox = pp - oy * p.Wo;
+          return true;
+        }
+        nimg = nimg_t; oy = oy0 + (r >> p.bw_log2); ox = ox0 + (r & (bw - 1));
+        return oy < p.Ho && ox < p.Wo && nimg < p.N;
+      });
     }
-    __syncwarp();
-  } else if (warp == TM_TMAWARP) {
-    // =========================== operand loader: four TMA boxes per K block (whole warp loops, one elected lane issues) =====
+  } else {
+    // =========================== producer: four TMA boxes per K block (whole warp loops, one elected lane issues) =====
     int s = 0; uint32_t ph = 1;
-    const uint32_t full_lead0 = CG == 2 ? mapa_rank(full_bar(0), 0) : full_bar(0);
-    for (int t = tile_first; t < total_tiles; t += tile_step) {
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       if (!needed(t)) continue;
       int nimg, oy0, ox0, n0;
       decode(t, nimg, oy0, ox0, n0);
@@ -589,12 +163,8 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
           const uint32_t a_hi = smem_base + (uint32_t)s * stage_bytes, a_mid = a_hi + a_bytes;
           const uint32_t b_hi = a_mid + a_bytes, b_mid = b_hi + b_bytes;
           const int x = ox0 * p.sx + sp.tdx[tap], y = oy0 * p.sy + sp.tdy[tap];
-          if (CG == 2)
-            tma_kblock_pair(full_lead0 + 8u * s, 2 * a_bytes + 2 * b_bytes, a_hi, a_mid, b_hi, b_mid, &sp.ta_hi, &sp.ta_mid, &p.tb_hi, &p.tb_mid,
-                            sp.c0 + cb * TC_BK, x, y, nimg, kb * TC_BK, n0 + (int)crank * (BN / 2));
-          else
-            tma_kblock(full_bar(s), 2 * a_bytes + 2 * b_bytes, a_hi, a_mid, b_hi, b_mid, &sp.ta_hi, &sp.ta_mid, &p.tb_hi, &p.tb_mid,
-                       sp.c0 + cb * TC_BK, x, y, nimg, kb * TC_BK, n0);
+          tma_kblock(full_bar(s), stage_bytes, a_hi, a_mid, b_hi, b_mid, &sp.ta_hi, &sp.ta_mid, &p.tb_hi, &p.tb_mid,
+                     sp.c0 + cb * TC_BK, x, y, nimg, kb * TC_BK, n0);
           if (++cb == sp.cblks) { cb = 0; ++tap; }
           if (++s == S) { s = 0; ph ^= 1u; }
         }
@@ -602,9 +172,6 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
     }
     __syncwarp();
   }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();             // pair: nobody leaves while the peer may still signal / read its smem
-  if (warp == TM_MMAWARP) { tc_fence_after(); tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols); }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -770,13 +337,12 @@ void make_w_tmap(CUtensorMap* m, const uint16_t* base, int kdim, int rows, int b
   MITB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for weights [%d x %d] box %d", (int)r, rows, kdim, bn);
 }
 
-// N tile width: minimise waves x tile time.  Tile time per K block = max(tensor floor 6*bn cycles, operand bytes over the
-// SM's share of L2 bandwidth ~42 B/clk); candidates split Cout into j equal tiles rounded up to 16.
-// cg = 2: tiles are 256-row pair tiles on sms/2 SM pairs, each CTA stages half of the weight tile.
-// Epilogue term: the accumulator is double buffered, so a tile costs max(main loop, epilogue) once the pipeline is full; the
-// epilogue drains 128 x bn elements at `epi` cycles per column (measured instruction counts of the packed epilogue: ~26 per
-// element with GELU + operand split, ~12 without, over 4 schedulers at ~0.7 issue efficiency).  MITB_CM="mode,epi_gelu,epi,fix"
-// overrides the constants (tools/cost_model_sweep.py).
+// N tile width: minimise waves x tile time.  Tile time = K blocks x max(tensor floor, operand bytes over the SM's share of L2
+// bandwidth) + epilogue + a fixed cost; candidates split Cout into j equal tiles rounded up to 32 (the wgmma widths instantiated,
+// at most 128).  Tensor floor: 3 x 128 x bn x 64 bf16 MACs per K block at the H100 SXM data-sheet dense bf16 rate (~2048 MAC per
+// clock per SM) = 12 bn cycles.  The epilogue runs after the main loop on the same warps (accumulators in registers), so the
+// two add.  The L2 share (42 B/clk) and the epilogue cycles per column are estimates, not measurements; MITB_CM=
+// "mode,epi_gelu,epi,fix" overrides the constants (mode 1: max instead of sum; tools/cost_model_sweep.py).
 struct CostModel { int mode; double epi_gelu, epi, fix; };
 const CostModel& cost_model() {
   static CostModel cm = {0, 40.0, 40.0, 600.0};
@@ -791,30 +357,21 @@ const CostModel& cost_model() {
   return cm;
 }
 
-int choose_bn(int Cout, long mtiles, int nkb, int sms, int cg, bool gelu, double* cost_out) {
+int choose_bn(int Cout, long mtiles, int nkb, int sms, bool gelu) {
   const CostModel& cm = cost_model();
-  double best = 1e30; int best_bn = 16;
-  const long units = sms / cg, mt = (mtiles + cg - 1) / cg;
+  double best = 1e30; int best_bn = 32;
   for (int j = 1; j <= 16; ++j) {
-    int bn = ((Cout + j - 1) / j + 15) & ~15;
-    if (bn > 256) continue;
-    if (bn < 16) bn = 16;
+    int bn = ((Cout + j - 1) / j + 31) & ~31;
+    if (bn > 128) continue;
     const long nt = (Cout + bn - 1) / bn;
-    const long waves = (mt * nt + units - 1) / units;
-    const double mma = 6.0 * bn, l2 = (32768.0 + 256.0 * bn / cg) / 42.0;
+    const long waves = (mtiles * nt + sms - 1) / sms;
+    const double mma = 12.0 * bn, l2 = (32768.0 + 256.0 * bn) / 42.0;
     const double main_loop = nkb * (mma > l2 ? mma : l2), epi = (gelu ? cm.epi_gelu : cm.epi) * bn;
     const double tile = (cm.mode == 1 ? (main_loop > epi ? main_loop : epi) : main_loop + epi) + cm.fix;
     const double cost = waves * tile;
     if (cost < best * 0.999) { best = cost; best_bn = bn; }
   }
-  if (cost_out) *cost_out = best;
   return best_bn;
-}
-
-int pair_mode_env() {        // MITB_CG2: 0 never, 1 when the cost model prefers it (default), 2 whenever legal
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("MITB_CG2"); v = e ? atoi(e) : 1; }
-  return v;
 }
 
 bool g_tma_enabled = true;
@@ -848,7 +405,7 @@ void launch_split(const View& in, const SplitView& sv, int coff, const float* in
   q.in_scale = in_scale; q.in_shift = in_shift; q.in_relu = in_relu;
   q.hi = sv.hi; q.mid = sv.mid; q.o_pitch = sv.C; q.o_coff = coff;
   const long total = (long)sv.N * sv.Hp * sv.Wp * (in.C / 8);
-  long blocks = (total + 255) / 256; if (blocks > 148L * 32) blocks = 148L * 32;
+  long blocks = (total + 255) / 256; if (blocks > device_sm_count() * 32L) blocks = device_sm_count() * 32L;
   if (blocks < 1) return;
   split_pad_kernel<<<(int)blocks, 256, 0, st>>>(q);
   count_launch();
@@ -860,7 +417,7 @@ void launch_split_halo(const SplitView& sv, int coff, int C, cudaStream_t st) {
   MITB_CHECK(sv.valid() && C % 8 == 0 && coff % 8 == 0 && sv.C % 8 == 0 && coff + C <= sv.C, "split halo: bad channel slice");
   MITB_CHECK(sv.pt < sv.H && sv.pl < sv.W && sv.Hp - sv.H - sv.pt < sv.H && sv.Wp - sv.W - sv.pl < sv.W, "split halo wider than the image");
   const long total = (long)sv.N * ((long)(sv.Hp - sv.H) * sv.Wp + (long)sv.H * (sv.Wp - sv.W)) * (C / 8);
-  long blocks = (total + 255) / 256; if (blocks > 148L * 8) blocks = 148L * 8;
+  long blocks = (total + 255) / 256; if (blocks > device_sm_count() * 8L) blocks = device_sm_count() * 8L;
   ProfScope ps("split_halo", 0.0, 4.0 * total * 8, st);
   split_halo_kernel<<<(int)blocks, 256, 0, st>>>(sv.hi, sv.mid, sv.N, sv.H, sv.W, sv.Hp, sv.Wp, sv.pt, sv.pl, sv.C, coff, C);
   count_launch();
@@ -937,7 +494,7 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
     static DeviceScratch g_stem;
     sv.hi = static_cast<uint16_t*>(g_stem.get(2 * sv.elems() * sizeof(uint16_t))); sv.mid = sv.hi + sv.elems();
     const long npix = (long)N * sv.Hp * sv.Wp;
-    long blocks = (npix + 255) / 256; if (blocks > 148L * 32) blocks = 148L * 32;
+    long blocks = (npix + 255) / 256; if (blocks > device_sm_count() * 32L) blocks = device_sm_count() * 32L;
     split_stem8_kernel<<<(int)blocks, 256, 0, st>>>(op.in.p, N, H, W, op.in.cs, op.in.coff, sv.Hp, sv.Wp, pt, pl, op.pad == PAD_REFLECT ? 1 : 0,
                                                     sv.hi, sv.mid);
     count_launch();
@@ -966,8 +523,10 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
   static PerDeviceOnce tma_attr;
   if (tma_attr.first()) {
 #define MITB_TMA_ATTR(A) \
-    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
+    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
+    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 96>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
+    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     MITB_TMA_ATTR(ACT_NONE) MITB_TMA_ATTR(ACT_RELU) MITB_TMA_ATTR(ACT_GELU) MITB_TMA_ATTR(ACT_SILU) MITB_TMA_ATTR(-1)
 #undef MITB_TMA_ATTR
   }
@@ -1028,26 +587,12 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
   p.nkb = kdim / TC_BK;
   // ---- N tile: fixed by the row-stat layout for the vocabulary head, otherwise chosen per launch against wave quantisation
   const long mtiles = (long)p.N * p.tiles_y * p.tiles_x;
-  int cg = 1;
-  if (op.stat_max) p.BN = op.tc_bn;
-  else {
-    double c1 = 0, c2 = 0;
-    const int bn1 = choose_bn(op.out.C, mtiles, p.nkb, num_sms, 1, op.act == ACT_GELU, &c1);
-    const int bn2 = choose_bn(op.out.C, mtiles, p.nkb, num_sms, 2, op.act == ACT_GELU, &c2);
-    const int mode = pair_mode_env();
-    // CTA pairs (cta_group::2) when the per-SM L2 budget, not the tensor pipe, bounds the tile and there are enough pair tiles
-    if (mtiles >= 2 && num_sms % 2 == 0 && (mode >= 2 || (mode == 1 && c2 < 0.97 * c1))) { cg = 2; p.BN = bn2; } else p.BN = bn1;
-  }
-  MITB_CHECK(p.BN >= 16 && p.BN <= 256 && p.BN % 16 == 0, "tma conv: bad BN %d", p.BN);
-  p.npad = (op.out.C + p.BN - 1) / p.BN * p.BN;
-  make_w_tmap(&p.tb_hi, stem ? op.w8h : padded_w ? op.whp : op.wh, kdim, op.tc_npad, p.BN / cg);
-  make_w_tmap(&p.tb_mid, stem ? op.w8m : padded_w ? op.wmp : op.wm, kdim, op.tc_npad, p.BN / cg);
-  p.out = op.out.p; p.oH = op.out.H; p.oW = op.out.W; p.out_cs = op.out.cs; p.out_coff = op.out.coff; p.Cout = op.out.C;
-  p.out_planar = op.out.planar; p.oy_mul = op.oy_mul; p.oy_add = op.oy_add; p.ox_mul = op.ox_mul; p.ox_add = op.ox_add;
-  p.add0 = op.add0.p; p.add0_cs = op.add0.cs; p.add0_coff = op.add0.coff; p.add0_planar = op.add0.planar;
-  p.add1 = op.add1.p; p.add1_cs = op.add1.cs; p.add1_coff = op.add1.coff; p.add1_planar = op.add1.planar;
-  p.scale = op.scale; p.shift = op.shift; p.mul1 = op.mul1; p.act = op.act;
-  p.stat_max = op.stat_max; p.stat_sum = op.stat_sum; p.stat_idx = op.stat_idx; p.stat_ld = op.stat_ld;
+  const int BN = op.stat_max ? op.tc_bn : choose_bn(op.out.C, mtiles, p.nkb, num_sms, op.act == ACT_GELU);
+  MITB_CHECK(BN >= 32 && BN <= 128 && BN % 32 == 0, "tma conv: bad BN %d", BN);
+  p.npad = (op.out.C + BN - 1) / BN * BN;
+  make_w_tmap(&p.tb_hi, stem ? op.w8h : padded_w ? op.whp : op.wh, kdim, op.tc_npad, BN);
+  make_w_tmap(&p.tb_mid, stem ? op.w8m : padded_w ? op.wmp : op.wm, kdim, op.tc_npad, BN);
+  fill_epi(p.e, op);
   if (op.out_sv.valid()) {
     const SplitView& o = op.out_sv;
     MITB_CHECK(!op.out.planar && op.out.C % 4 == 0 && !op.stat_max && op.oy_mul == 1 && op.ox_mul == 1 && op.oy_add == 0 && op.ox_add == 0 &&
@@ -1056,25 +601,8 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
                (!op.add0.p || (!op.add0.planar && ((op.add0.cs | op.add0.coff) & 3) == 0)) &&
                (!op.add1.p || (!op.add1.planar && ((op.add1.cs | op.add1.coff) & 3) == 0)),
                "tma conv: out_sv needs an NHWC output on the conv's own pixel grid");
-    MITB_CHECK((size_t)o.N * o.Hp * o.Wp < ((size_t)1 << 32), "tma conv: out_sv too large for 32-bit pixel indices");
-    p.os_hi = o.hi; p.os_mid = o.mid; p.os_pitch = o.C; p.os_coff = op.out_sv_coff; p.os_Hp = o.Hp; p.os_Wp = o.Wp; p.os_pt = o.pt; p.os_pl = o.pl;
-    p.os_scale = op.os_scale; p.os_shift = op.os_shift; p.os_relu = op.os_relu;
-    if (!op.out.p) { p.oH = op.Ho; p.oW = op.Wo; }
+    if (!op.out.p) { p.e.oH = op.Ho; p.e.oW = op.Wo; }
   } else MITB_CHECK(op.out.p || op.stat_max, "tma conv: no output");
-  {
-    auto al16 = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
-    p.fast = !op.stat_max && !op.out.planar && op.out.C % 4 == 0 && ((op.out.cs | op.out.coff) & 3) == 0 && al16(op.out.p) &&
-             (!op.add0.p || (!op.add0.planar && ((op.add0.cs | op.add0.coff) & 3) == 0 && al16(op.add0.p))) &&
-             (!op.add1.p || (!op.add1.planar && ((op.add1.cs | op.add1.coff) & 3) == 0 && al16(op.add1.p))) && !(op.add0.p && op.add1.p) &&
-             (size_t)op.out.N * p.oH * p.oW * (size_t)(op.out.p ? op.out.cs : 1) < ((size_t)1 << 31) &&
-             (!op.add0.p || (size_t)op.out.N * p.oH * p.oW * (size_t)op.add0.cs < ((size_t)1 << 31)) &&
-             (!op.add1.p || (size_t)op.out.N * p.oH * p.oW * (size_t)op.add1.cs < ((size_t)1 << 31)) &&
-             (!p.os_hi || (size_t)op.out_sv.N * op.out_sv.Hp * op.out_sv.Wp * (size_t)op.out_sv.C < ((size_t)1 << 31)) && al16(op.scale) && al16(op.shift) && al16(op.mul1) && al16(op.os_scale) && al16(op.os_shift) &&
-             (!p.os_hi || (((uintptr_t)p.os_hi | (uintptr_t)p.os_mid) & 7) == 0);
-    static int env = -1;
-    if (env < 0) { const char* e = getenv("MITB_SLOW_EPILOGUE"); env = (e && atoi(e)) ? 1 : 0; }
-    if (env) p.fast = 0;
-  }
   MITB_CHECK(!op.stat_max || op.stat_ld == 2 * (op.tc_npad / op.tc_bn), "tma conv: stat_ld must equal conv_stat_blocks(op)");
   if (op.need_px && !op.stat_max) {
     // reduce the pixel-level hint to this launch's tile grid (one tiny launch; the scratch is per device and stream ordered)
@@ -1084,25 +612,21 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
     count_launch();
     p.tile_need = tn;
   }
-  int cols = 32; while (cols < p.BN) cols <<= 1;
-  p.tmem_cols = 2 * cols;
-  const size_t stage_bytes = 2 * (size_t)TC_BM * 128 + 2 * (size_t)(p.BN / cg) * 128;
-  const size_t epi_bytes = (size_t)TM_EWARPS * 32 * 20 * sizeof(float);
-  int stages = (int)((227 * 1024 - 1024 - 256 - epi_bytes) / stage_bytes); if (stages > 6) stages = 6;
+  const size_t stage_bytes = 2 * (size_t)TC_BM * 128 + 2 * (size_t)BN * 128;
+  int stages = (int)((227 * 1024 - 1024 - 256) / stage_bytes); if (stages > 6) stages = 6;
   MITB_CHECK(stages >= 2, "tma conv: tile does not fit shared memory");
   p.stages = stages;
-  const size_t smem = stages * stage_bytes + (2 * stages + 6) * 8 + epi_bytes + 1024;
-  const long total_tiles = ((mtiles + cg - 1) / cg) * (p.npad / p.BN);
-  const long units = num_sms / cg;
-  const int grid = (int)(total_tiles < units ? total_tiles : units) * cg;
-  cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(TM_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = (unsigned)cg; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-#define MITB_TMA_LAUNCH(A) \
-  do { if (cg == 2) CUDA_OK(cudaLaunchKernelEx(&cfg, conv_tma_kernel<A, 2>, p)); else CUDA_OK(cudaLaunchKernelEx(&cfg, conv_tma_kernel<A, 1>, p)); } while (0)
-  switch (op.stat_max ? ACT_NONE : p.act) {
+  const size_t smem = stages * stage_bytes + 2 * stages * 8 + 1024;
+  const long total_tiles = mtiles * (p.npad / BN);
+  const int grid = (int)(total_tiles < num_sms ? total_tiles : num_sms);      // persistent: one CTA per SM
+#define MITB_TMA_LAUNCH(A)                                                              \
+  switch (BN) {                                                                        \
+    case 32: conv_tma_kernel<A, 32><<<grid, TM_THREADS, smem, st>>>(p); break;          \
+    case 64: conv_tma_kernel<A, 64><<<grid, TM_THREADS, smem, st>>>(p); break;          \
+    case 96: conv_tma_kernel<A, 96><<<grid, TM_THREADS, smem, st>>>(p); break;          \
+    default: conv_tma_kernel<A, 128><<<grid, TM_THREADS, smem, st>>>(p); break;         \
+  }
+  switch (op.stat_max ? ACT_NONE : op.act) {
     case ACT_NONE: MITB_TMA_LAUNCH(ACT_NONE); break;
     case ACT_RELU: MITB_TMA_LAUNCH(ACT_RELU); break;
     case ACT_GELU: MITB_TMA_LAUNCH(ACT_GELU); break;

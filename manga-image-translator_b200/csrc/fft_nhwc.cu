@@ -37,13 +37,12 @@ struct FftNDev { int n, nst, nbt; int radix[kMaxSt]; const float2* tw; const uin
 
 #include "tc_common.cuh"
 
-// complex arithmetic on the packed fp32x2 pipe of sm_100 (add.f32x2 / fma.rn.f32x2): one instruction per complex add / subtract,
-// two per complex multiply - the butterflies are instruction-issue bound (ncu), so halving their FP instruction count pays
+// complex arithmetic on fp32 pairs (ffma2 / fmul2 / fadd2 of mitb_internal.h): one fused multiply-add per component
 __device__ __forceinline__ float2 cmulf(float2 a, float2 b) {
-  return __ffma2_rn(make_float2(a.x, a.x), b, __fmul2_rn(make_float2(a.y, a.y), make_float2(-b.y, b.x)));
+  return ffma2(make_float2(a.x, a.x), b, fmul2(make_float2(a.y, a.y), make_float2(-b.y, b.x)));
 }
-__device__ __forceinline__ float2 caddf(float2 a, float2 b) { return __fadd2_rn(a, b); }
-__device__ __forceinline__ float2 csubf(float2 a, float2 b) { return __ffma2_rn(b, make_float2(-1.f, -1.f), a); }
+__device__ __forceinline__ float2 caddf(float2 a, float2 b) { return fadd2(a, b); }
+__device__ __forceinline__ float2 csubf(float2 a, float2 b) { return ffma2(b, make_float2(-1.f, -1.f), a); }
 // multiply by -i (forward) or +i (inverse)
 __device__ __forceinline__ float2 rot90(float2 a, bool inv) { return inv ? make_float2(-a.y, a.x) : make_float2(a.y, -a.x); }
 
@@ -63,8 +62,8 @@ __device__ __forceinline__ void dft4(float2& a0, float2& a1, float2& a2, float2&
 template <bool INV>
 __device__ __forceinline__ void dft3(float2& a0, float2& a1, float2& a2) {
   const float2 t1 = caddf(a1, a2);
-  const float2 t2 = __ffma2_rn(t1, make_float2(-0.5f, -0.5f), a0);
-  const float2 t3 = __fmul2_rn(csubf(a1, a2), make_float2(0.86602540378443864676f, 0.86602540378443864676f));
+  const float2 t2 = ffma2(t1, make_float2(-0.5f, -0.5f), a0);
+  const float2 t3 = fmul2(csubf(a1, a2), make_float2(0.86602540378443864676f, 0.86602540378443864676f));
   // forward: y1 = t2 - i t3, y2 = t2 + i t3 ; inverse: swapped
   const float2 y1 = make_float2(t2.x + t3.y, t2.y - t3.x), y2 = make_float2(t2.x - t3.y, t2.y + t3.x);
   a0 = caddf(a0, t1);
@@ -322,7 +321,7 @@ __global__ void __launch_bounds__(FT, 3) irfft_rows_nhwc_kernel(const __grid_con
   const bool ok = 2 * pair < p.C;
   load_tables(p.pl, tw, rev, bt);
   const float2* src = reinterpret_cast<const float2*>(p.in) + (size_t)row * p.w2 * p.C;
-#pragma unroll 4                                       // several rows' loads in flight per warp (ncu: this kernel waited on one load at a time)
+#pragma unroll 4                                       // several rows' loads in flight per warp
   for (int k = warp; k < p.w2; k += FW) {
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (ok) v = __ldg(reinterpret_cast<const float4*>(src + (size_t)k * p.C + 2 * pair));

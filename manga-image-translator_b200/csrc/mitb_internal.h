@@ -325,6 +325,11 @@ inline int device_sm_count() {
   return sms[dev];
 }
 
+// fp32 pairs: two independent round-to-nearest operations per call (the fused multiply-add is one rounding, like fmaf)
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+
 extern unsigned long g_launch_epoch;     // bumped by EVERY kernel launch of the library (conv_tma.cu's split reuse keys on it)
 inline void count_launch() { ++g_launch_epoch; if (g_launch_counter) ++*g_launch_counter; }
 

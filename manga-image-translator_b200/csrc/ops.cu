@@ -92,10 +92,9 @@ void launch_layernorm(const View& in, const View& out, const float* w, const flo
 // output pixels of one row; the C/4 threads with the same threadIdx.y jointly normalise those 8 pixels.
 constexpr int DW_TX = 8;
 
-// ncu (r02, C = 512): the first version of this kernel was bound by instruction issue, not by memory - 31 M warp instructions
-// for 9.6 M warp-FMAs: 64-bit address arithmetic and a bounds predicate per input pixel, scalar FMAs.  This version keeps the same
-// tiling (same summation order per output: bias, then taps in (dy, dx) order) but runs the taps on the packed fp32x2 pipe (two
-// channels per instruction), addresses the input with 32-bit element offsets from one base pointer, and takes a predicate-free
+// Written for instruction count (the straightforward version, with 64-bit address arithmetic, a bounds predicate per input pixel
+// and scalar FMAs, is bound by instruction issue rather than memory).  The tiling fixes the summation order per output (bias, then
+// taps in (dy, dx) order); the taps run as fp32 pairs (two channels per step), addresses the input with 32-bit element offsets from one base pointer, and takes a predicate-free
 // path for tiles that do not touch the left / right image border (CTA-uniform).
 __device__ __forceinline__ void dw_taps(float2 (&acc)[DW_TX][2], const float4 v, const float2 (&wv)[7][2], int j) {
   const float2 lo = make_float2(v.x, v.y), hi = make_float2(v.z, v.w);
@@ -103,8 +102,8 @@ __device__ __forceinline__ void dw_taps(float2 (&acc)[DW_TX][2], const float4 v,
   for (int dx = 0; dx < 7; ++dx) {
     const int i = j - dx;                    // output pixel fed by input pixel j through tap dx (resolved at compile time)
     if (i >= 0 && i < DW_TX) {
-      acc[i][0] = __ffma2_rn(lo, wv[dx][0], acc[i][0]);
-      acc[i][1] = __ffma2_rn(hi, wv[dx][1], acc[i][1]);
+      acc[i][0] = ffma2(lo, wv[dx][0], acc[i][0]);
+      acc[i][1] = ffma2(hi, wv[dx][1], acc[i][1]);
     }
   }
 }
@@ -280,7 +279,7 @@ __global__ void avgpool_kernel(const float* in, int in_cs, int in_coff, float* o
 void launch_avgpool(const View& in, const View& out, int mode, cudaStream_t st) {
   MITB_CHECK(in.C % 4 == 0 && in.cs % 4 == 0 && in.coff % 4 == 0 && out.cs % 4 == 0 && out.coff % 4 == 0, "avgpool alignment");
   const long total = (long)out.N * out.H * out.W * (in.C / 4);
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   avgpool_kernel<<<blocks, 256, 0, st>>>(in.p, in.cs, in.coff, out.p, out.cs, out.coff, in.N, in.H, in.W, in.C / 4,
                                          out.H, out.W, mode);
   LAUNCH_END();
@@ -298,7 +297,7 @@ __global__ void nchw_to_nhwc_kernel(const float* src, int N, int C, int H, int W
 }
 void launch_nchw_to_nhwc(const float* src, int N, int C, int H, int W, const View& dst, cudaStream_t st) {
   const long total = (long)N * H * W;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   nchw_to_nhwc_kernel<<<blocks, 256, 0, st>>>(src, N, C, H, W, dst.p, dst.cs, dst.coff, dst.C);
   LAUNCH_END();
 }
@@ -312,7 +311,7 @@ __global__ void nhwc_to_nchw_kernel(const float* src, int cs, int coff, int N, i
 }
 void launch_nhwc_to_nchw(const View& src, float* dst, cudaStream_t st) {
   const long total = (long)src.N * src.C * src.H * src.W;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   nhwc_to_nchw_kernel<<<blocks, 256, 0, st>>>(src.p, src.cs, src.coff, src.N, src.C, src.H, src.W, dst);
   LAUNCH_END();
 }
@@ -336,7 +335,7 @@ __global__ void u8_to_nhwc_kernel(const uint8_t* src, long npix, int C, float* d
 void launch_u8_to_nhwc(const uint8_t* src, int N, int H, int W, int C, const View& dst, float mul, float add,
                        int div_first, cudaStream_t st) {
   const long npix = (long)N * H * W;
-  int blocks = (int)((npix + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((npix + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   u8_to_nhwc_kernel<<<blocks, 256, 0, st>>>(src, npix, C, dst.p, dst.cs, dst.coff, dst.C, mul, add, div_first);
   LAUNCH_END();
 }
@@ -362,7 +361,7 @@ __global__ void affine_act_kernel(const float* in, int in_cs, int in_coff, float
 }
 void launch_affine_act(const View& in, const View& out, const float* scale, const float* shift, int act, cudaStream_t st) {
   const long total = (long)in.pixels() * in.C;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   affine_act_kernel<<<blocks, 256, 0, st>>>(in.p, in.cs, in.coff, out.p, out.cs, out.coff, (long)in.pixels(), in.C, scale, shift, act);
   LAUNCH_END();
 }
@@ -372,7 +371,7 @@ void launch_affine_act(const View& in, const View& out, const float* scale, cons
 // (line, head); K and V of that head staged in shared memory (stride hd+1), one warp per query row,
 // softmax(q.k / sqrt(hd)) v with no padding mask.
 // gridDim.y row blocks per (line, head): each CTA re-stages K/V (L2 resident) and takes every gridDim.y-th group of query rows,
-// so the 128 (line, head) pairs of a 16-line chunk fill all 148 SMs several CTAs deep instead of 128 SMs one CTA deep.
+// so the 128 (line, head) pairs of a 16-line chunk fill all SMs (132 on an H100) several CTAs deep instead of 128 SMs one CTA deep.
 __global__ void attention_kernel(const float* qk, const float* v, float* out, int T, int heads, int hd, float scale) {
   extern __shared__ float sm[];
   const int D = heads * hd;
@@ -417,7 +416,7 @@ __global__ void attention_kernel(const float* qk, const float* v, float* out, in
 
 // head_dim = 40 (the OCR encoder, model_48px_ctc.py:432): same decomposition, restructured for instruction count - the generic kernel
 // above spends two shared-memory loads per FMA.  K / V rows are padded to 44 floats so that a row is ten aligned LDS.128 (conflict
-// free per quarter warp), q lives in registers, the dot products and the P.V accumulation run on the packed fp32x2 pipe, and P.V is
+// free per quarter warp), q lives in registers, the dot products and the P.V accumulation run on fp32 pairs, and P.V is
 // split over the keys (each lane accumulates its own keys into 40 registers, the 32 partial vectors are summed through shared memory).
 constexpr int AT_HD = 40, AT_LD = 44;
 __global__ void __launch_bounds__(256) attention40_kernel(const float* __restrict__ qk, const float* __restrict__ v, float* __restrict__ out, int T,
@@ -451,8 +450,8 @@ __global__ void __launch_bounds__(256) attention40_kernel(const float* __restric
 #pragma unroll
       for (int i = 0; i < AT_HD / 4; ++i) {
         const float4 a = kr[i];
-        s2 = __ffma2_rn(q[2 * i], make_float2(a.x, a.y), s2);
-        s2 = __ffma2_rn(q[2 * i + 1], make_float2(a.z, a.w), s2);
+        s2 = ffma2(q[2 * i], make_float2(a.x, a.y), s2);
+        s2 = ffma2(q[2 * i + 1], make_float2(a.z, a.w), s2);
       }
       const float s = (s2.x + s2.y) * scale;
       P[j] = s; mx = fmaxf(mx, s);
@@ -470,8 +469,8 @@ __global__ void __launch_bounds__(256) attention40_kernel(const float* __restric
 #pragma unroll
       for (int i = 0; i < AT_HD / 4; ++i) {
         const float4 a = vr[i];
-        acc[2 * i] = __ffma2_rn(make_float2(e, e), make_float2(a.x, a.y), acc[2 * i]);
-        acc[2 * i + 1] = __ffma2_rn(make_float2(e, e), make_float2(a.z, a.w), acc[2 * i + 1]);
+        acc[2 * i] = ffma2(make_float2(e, e), make_float2(a.x, a.y), acc[2 * i]);
+        acc[2 * i + 1] = ffma2(make_float2(e, e), make_float2(a.z, a.w), acc[2 * i + 1]);
       }
     }
 #pragma unroll
@@ -534,7 +533,7 @@ __global__ void lama_pack_kernel(const float* img, const float* mask, int N, lon
 }
 void launch_lama_pack_input(const float* img, const float* mask, int N, int H, int W, const View& dst, cudaStream_t st) {
   const long total = (long)N * H * W;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   lama_pack_kernel<<<blocks, 256, 0, st>>>(img, mask, N, (long)H * W, dst.p, dst.cs, dst.coff, dst.C);
   LAUNCH_END();
 }
@@ -595,7 +594,7 @@ __global__ void lama_blend_kernel(const float* pred, const float* img, const flo
 void launch_lama_blend(const View& pred, const float* img, const float* mask, float* out, cudaStream_t st) {
   MITB_CHECK(pred.planar && pred.C == 3 && pred.cs == 3 && pred.coff == 0, "blend expects a planar 3-channel prediction");
   const long total = (long)pred.N * 3 * pred.H * pred.W;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   lama_blend_kernel<<<blocks, 256, 0, st>>>(pred.p, img, mask, out, pred.N, (long)pred.H * pred.W);
   LAUNCH_END();
 }
@@ -621,7 +620,7 @@ __global__ void lama_pack_u8_kernel(const uint8_t* img, const uint8_t* mask, lon
 }
 void launch_lama_pack_u8(const uint8_t* img, const uint8_t* mask, int H, int W, const View& dst, float* maskf, cudaStream_t st) {
   const long total = (long)H * W;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   lama_pack_u8_kernel<<<blocks, 256, 0, st>>>(img, mask, total, dst.p, dst.cs, dst.coff, dst.C, maskf);
   LAUNCH_END();
 }
@@ -643,7 +642,7 @@ __global__ void lama_blend_u8_kernel(const float* pred, const uint8_t* img, cons
 void launch_lama_blend_u8(const View& pred, const uint8_t* img, const uint8_t* mask, uint8_t* out, int composite, cudaStream_t st) {
   MITB_CHECK(pred.planar && pred.C == 3 && pred.cs == 3 && pred.coff == 0 && pred.N == 1, "blend_u8 expects one planar 3-channel prediction");
   const long total = (long)pred.H * pred.W;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   lama_blend_u8_kernel<<<blocks, 256, 0, st>>>(pred.p, img, mask, out, total, composite);
   LAUNCH_END();
 }
@@ -742,7 +741,7 @@ void launch_mpe_add(const View& x, const int* rel_pos, const int* direct, int th
                     const float* dirw, float a5, float a6, cudaStream_t st) {
   MITB_CHECK(x.C == 64 && x.cs % 4 == 0 && x.coff % 4 == 0, "mpe_add expects the 64-channel stem output");
   const long total = (long)x.pixels() * 16;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 32) blocks = 148 * 32;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
   mpe_add_kernel<<<blocks, 256, 0, st>>>(x.p, x.cs, x.coff, x.N, x.H, x.W, rel_pos, direct, th, tw, mask, table, dirw, a5, a6);
   LAUNCH_END();
 }

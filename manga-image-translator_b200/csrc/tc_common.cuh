@@ -1,7 +1,43 @@
-// Device helpers shared by the tcgen05 convolution kernels (conv_tc.cu: register-gather producers; conv_tma.cu: TMA-fed
-// operands): mbarrier / TMA / tcgen05 / TMEM wrappers, the UMMA shared-memory descriptor, the bf16 hi/mid split and the
-// epilogue activations.  Included inside namespace mitb { namespace { ... } } of each translation unit.
+// Device helpers shared by the wgmma convolution kernels (conv_tc.cu: register-gather producers; conv_tma.cu: TMA-fed
+// operands): mbarrier / TMA / wgmma wrappers, the shared-memory matrix descriptor, the bf16 hi/mid split, the epilogue
+// activations and the epilogue itself.  Included inside namespace mitb { namespace { ... } } of each translation unit.
 #pragma once
+
+// What the epilogue needs to know about the output side of a conv (ConvOp fields, see mitb_internal.h)
+struct EpiParams {
+  float* out; int oH, oW, out_cs, out_coff, Cout, out_planar, oy_mul, oy_add, ox_mul, ox_add;
+  int Ho, Wo, M;                                              // logical output grid, rows of the GEMM
+  const float* add0; int add0_cs, add0_coff, add0_planar;
+  const float* add1; int add1_cs, add1_coff, add1_planar;
+  const float* scale; const float* shift; const float* mul1; int act;
+  float* stat_max; float* stat_sum; int* stat_idx; int stat_ld;     // fused log-softmax/argmax partials (vocabulary head)
+  // split output (ConvOp::out_sv): bf16 hi / mid at [((n*os_Hp + y + os_pt)*os_Wp + x + os_pl)*os_pitch + os_coff + c] (null: none)
+  uint16_t* os_hi; uint16_t* os_mid; int os_pitch, os_coff, os_Hp, os_Wp, os_pt, os_pl;
+  const float* os_scale; const float* os_shift; int os_relu;  // consumer prologue applied before splitting
+  float* partial; int npad;                                   // split-K: partial sums [splits][M][npad] (null: none)
+  int vec2;                                                   // NHWC, even strides / offsets, 8-byte aligned operands, Cout even
+};
+
+inline void fill_epi(EpiParams& e, const ConvOp& op) {
+  memset(&e, 0, sizeof(e));
+  e.out = op.out.p; e.oH = op.out.H; e.oW = op.out.W; e.out_cs = op.out.cs; e.out_coff = op.out.coff; e.Cout = op.out.C;
+  e.out_planar = op.out.planar; e.oy_mul = op.oy_mul; e.oy_add = op.oy_add; e.ox_mul = op.ox_mul; e.ox_add = op.ox_add;
+  e.Ho = op.Ho; e.Wo = op.Wo; e.M = op.in.N * op.Ho * op.Wo;
+  e.add0 = op.add0.p; e.add0_cs = op.add0.cs; e.add0_coff = op.add0.coff; e.add0_planar = op.add0.planar;
+  e.add1 = op.add1.p; e.add1_cs = op.add1.cs; e.add1_coff = op.add1.coff; e.add1_planar = op.add1.planar;
+  e.scale = op.scale; e.shift = op.shift; e.mul1 = op.mul1; e.act = op.act;
+  e.stat_max = op.stat_max; e.stat_sum = op.stat_sum; e.stat_idx = op.stat_idx; e.stat_ld = op.stat_ld;
+  if (op.out_sv.valid()) {
+    const SplitView& o = op.out_sv;
+    e.os_hi = o.hi; e.os_mid = o.mid; e.os_pitch = o.C; e.os_coff = op.out_sv_coff; e.os_Hp = o.Hp; e.os_Wp = o.Wp; e.os_pt = o.pt; e.os_pl = o.pl;
+    e.os_scale = op.os_scale; e.os_shift = op.os_shift; e.os_relu = op.os_relu;
+  }
+  auto al8 = [](const void* q) { return ((uintptr_t)q & 7) == 0; };
+  auto nhwc_ok = [&](const View& v) { return !v.p || (!v.planar && ((v.cs | v.coff) & 1) == 0 && al8(v.p)); };
+  e.vec2 = !op.out.planar && op.out.C % 2 == 0 && nhwc_ok(op.out) && nhwc_ok(op.add0) && nhwc_ok(op.add1) && al8(op.scale) && al8(op.shift) &&
+           al8(op.mul1) && al8(op.os_scale) && al8(op.os_shift) && (!e.os_hi || ((e.os_pitch | e.os_coff) & 1) == 0) &&
+           (!e.os_hi || (((uintptr_t)e.os_hi | (uintptr_t)e.os_mid) & 3) == 0);
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -42,49 +78,72 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap
                ::"r"(smem_dst), "l"(map), "r"(bar), "r"(x), "r"(y) : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- wgmma (warpgroup MMA, sm_90a): D[64 x N] (fp32, registers of the 128 threads of a warpgroup) += A[64 x 16] * B[16 x N],
+// both operands K-major in shared memory.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across wgmma_wait / wgmma_fence
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, int accumulate);
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float (&d)[16], uint64_t da, uint64_t db, int accumulate) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t da, uint64_t db, int accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-__device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+template <> __device__ __forceinline__ void wgmma_bf16<96>(float (&d)[48], uint64_t da, uint64_t db, int accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-__device__ __forceinline__ float4 lds128(uint32_t saddr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr) : "memory");
-  return v;
+template <> __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t da, uint64_t db, int accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory matrix descriptor: K-major operand, 128-byte swizzle, rows of 128 B, 8-row groups 1024 B apart.
+// wgmma shared-memory matrix descriptor: K-major operand, 128-byte swizzle, rows of 128 B, 8-row groups 1024 B apart.
 //   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major, 1) | [32,46) stride byte
-//   offset >> 4 (1024 >> 4) | [46,48) descriptor version 1 (sm_100) | [61,64) layout type 2 = SWIZZLE_128B
+//   offset >> 4 (1024 >> 4) | [62,64) layout type 1 = SWIZZLE_128B.  A 16-element step along K inside the swizzle row is +32 B
+//   of start address (+2 in the descriptor).
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+
+// One K block (64 channels) of the bf16x3 product for this warpgroup: for each 16-wide k step Ah*Bh, Ah*Bm, Am*Bh
+template <int BN>
+__device__ __forceinline__ void wgmma_kblock_x3(float (&acc)[BN / 2], uint64_t dah, uint64_t dam, uint64_t dbh, uint64_t dbm, bool first) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint64_t adv = (uint64_t)(2 * k);
+    wgmma_bf16<BN>(acc, dah + adv, dbh + adv, (first && k == 0) ? 0 : 1);
+    wgmma_bf16<BN>(acc, dah + adv, dbm + adv, 1);
+    wgmma_bf16<BN>(acc, dam + adv, dbh + adv, 1);
+  }
 }
 
 __device__ __forceinline__ float apply_act_tc(float v, int act) {
@@ -149,52 +208,6 @@ __device__ __forceinline__ float gelu_fast(float x) {
   return 0.5f * x * (1.f + copysignf(erf_abs, x));
 }
 
-// The same GELU on the packed fp32x2 pipe of sm_100 (fma.rn.f32x2 / mul.f32x2), two elements per call, rewritten so that no
-// sign transfer is needed:  gelu(x) = max(x, 0) - 0.5 |x| p(t) exp(-z^2),  z = |x| / sqrt 2,  t = 1 / (1 + 0.3275911 z)
-// (x >= 0: x (1 - pe/2); x < 0: x pe/2 = -|x| pe/2).  The polynomial coefficients carry the factor -1/2; exp(-z^2) =
-// ex2(-(|x| sqrt(log2(e)/2))^2).  19 instructions per PAIR (4 of them MUFU) against 17 per element for gelu_fast.
-__device__ __forceinline__ float2 gelu_fast2(float2 x) {
-  const float2 ax = make_float2(fabsf(x.x), fabsf(x.y));
-  const float2 d = __ffma2_rn(ax, make_float2(0.23164189028714973f, 0.23164189028714973f), make_float2(1.f, 1.f));   // 0.3275911 / sqrt 2
-  float2 t;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t.x) : "f"(d.x));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t.y) : "f"(d.y));
-  float2 pl = __ffma2_rn(t, make_float2(-0.5307027145f, -0.5307027145f), make_float2(0.7265760135f, 0.7265760135f));
-  pl = __ffma2_rn(pl, t, make_float2(-0.7107068705f, -0.7107068705f));
-  pl = __ffma2_rn(pl, t, make_float2(0.142248368f, 0.142248368f));
-  pl = __ffma2_rn(pl, t, make_float2(-0.127414796f, -0.127414796f));
-  pl = __fmul2_rn(pl, t);                                   // -p(t) / 2
-  const float2 u = __fmul2_rn(ax, make_float2(0.84932180028801904f, 0.84932180028801904f));      // sqrt(log2(e) / 2)
-  const float2 w = __fmul2_rn(u, u);
-  float2 e;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(-w.x));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(-w.y));
-  const float2 h = __fmul2_rn(ax, pl);
-  return __ffma2_rn(h, e, make_float2(fmaxf(x.x, 0.f), fmaxf(x.y, 0.f)));
-}
-
-// split 4 fp32 values (two packed pairs) into bf16 hi / mid packs with the remainder on the packed pipe: 10 instructions
-__device__ __forceinline__ void split4p(float2 a, float2 b, uint2& hi, uint2& mid) {
-  const __nv_bfloat162 h0 = __floats2bfloat162_rn(a.x, a.y), h1 = __floats2bfloat162_rn(b.x, b.y);
-  const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&h0), b1 = *reinterpret_cast<const uint32_t*>(&h1);
-  const float2 m1 = make_float2(-1.f, -1.f);
-  const float2 r0 = __ffma2_rn(make_float2(__uint_as_float(b0 << 16), __uint_as_float(b0 & 0xffff0000u)), m1, a);   // a - hi, exact
-  const float2 r1 = __ffma2_rn(make_float2(__uint_as_float(b1 << 16), __uint_as_float(b1 & 0xffff0000u)), m1, b);
-  const __nv_bfloat162 q0 = __floats2bfloat162_rn(r0.x, r0.y), q1 = __floats2bfloat162_rn(r1.x, r1.y);
-  hi = make_uint2(b0, b1);
-  mid = make_uint2(*reinterpret_cast<const uint32_t*>(&q0), *reinterpret_cast<const uint32_t*>(&q1));
-}
-
-template <int ACT>
-__device__ __forceinline__ float act_t(float v, int act_rt);
-template <int ACT>
-__device__ __forceinline__ float2 act_t2(float2 v, int act_rt) {
-  if (ACT == ACT_NONE) return v;
-  if (ACT == ACT_RELU) return make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
-  if (ACT == ACT_GELU) return gelu_fast2(v);
-  return make_float2(act_t<ACT>(v.x, act_rt), act_t<ACT>(v.y, act_rt));
-}
-
 template <int ACT>
 __device__ __forceinline__ float act_t(float v, int act_rt) {
   if (ACT == ACT_NONE) return v;
@@ -204,3 +217,128 @@ __device__ __forceinline__ float act_t(float v, int act_rt) {
   return apply_act_tc(v, act_rt);               // ACT == -1: rare activations, runtime switch
 }
 
+
+// split 2 fp32 values into packed bf16 hi / mid pairs
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& mid) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h);
+  const __nv_bfloat162 m = __floats2bfloat162_rn(a - __uint_as_float(hb << 16), b - __uint_as_float(hb & 0xffff0000u));
+  hi = hb; mid = *reinterpret_cast<const uint32_t*>(&m);
+}
+
+// (max, first argmax, sum exp) partials of the vocabulary head: merge b into a
+__device__ __forceinline__ void stat_merge(float& am, float& as, int& ai, float bm, float bs, int bi) {
+  const float m = fmaxf(am, bm);
+  if (m == -INFINITY) { ai = min(ai, bi); return; }
+  as = as * expf(am - m) + bs * expf(bm - m);
+  ai = am > bm ? ai : bm > am ? bi : min(ai, bi);
+  am = m;
+}
+
+// Epilogue of one 128 x BN output tile from the wgmma accumulator fragments.  Warp w of warpgroup g holds rows
+// 64 g + 16 (w % 4) + lane / 4 (registers 4j, 4j+1) and the row 8 below it (4j+2, 4j+3), columns 8 j + 2 (lane % 4) + {0, 1}:
+// a warp store covers 8 rows x 32 contiguous bytes, whole sectors.  rowpix(r, nimg, oy, ox) maps tile row r to its output pixel
+// (false: outside).  Modes: vocabulary-head row statistics, split-K partial sums, or the fused elementwise chain
+// v = acc (+add0) ; v = v*scale+shift ; act ; *mul1 ; +add1 -> fp32 out and / or the consumer's bf16 hi / mid operands.
+template <int ACT, int BN, class RowPix>
+__device__ __forceinline__ void epilogue_tile(const EpiParams& e, const float (&acc)[BN / 2], int row0, int n0, int z, RowPix rowpix) {
+  const int lane = threadIdx.x & 31;
+  const int cl = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    int nimg = 0, oy = 0, ox = 0;
+    const bool ok = rowpix(row0 + 8 * h, nimg, oy, ox);
+    if (e.stat_max) {
+      // online (max, first argmax, sum exp) per column half of the N tile over this thread's columns, then over the 4 lanes of
+      // the row (model_48px_ctc.py:460-461); the logits never leave the registers
+      constexpr int kHalf = ((BN / 16 + 1) / 2) * 16;
+      float bm[2] = {-INFINITY, -INFINITY}, bs[2] = {0.f, 0.f}; int bi[2] = {0x7fffffff, 0x7fffffff};
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const int cc = 8 * j + cl + q, c = n0 + cc, hf = cc < kHalf ? 0 : 1;
+          if (c < e.Cout) {
+            const float x = acc[4 * j + 2 * h + q] + (e.shift ? __ldg(e.shift + c) : 0.f);
+            if (x > bm[hf]) { bs[hf] = bs[hf] * expf(bm[hf] - x) + 1.f; bm[hf] = x; bi[hf] = c; }
+            else bs[hf] += expf(x - bm[hf]);
+          }
+        }
+      }
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1)
+          stat_merge(bm[hf], bs[hf], bi[hf], __shfl_xor_sync(0xffffffffu, bm[hf], o), __shfl_xor_sync(0xffffffffu, bs[hf], o),
+                     __shfl_xor_sync(0xffffffffu, bi[hf], o));
+        if (ok && (lane & 3) == 0) {
+          const size_t o = (((size_t)nimg * e.Ho + oy) * e.Wo + ox) * e.stat_ld + (n0 / BN) * 2 + hf;
+          e.stat_max[o] = bm[hf]; e.stat_sum[o] = bs[hf]; e.stat_idx[o] = bi[hf];
+        }
+      }
+      continue;
+    }
+    if (!ok) continue;
+    if (e.partial) {
+      // split-K partial: raw accumulators to partial[z][m][npad]
+      float* dst = e.partial + ((size_t)z * e.M + ((size_t)nimg * e.Ho + oy) * e.Wo + ox) * e.npad + n0 + cl;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      continue;
+    }
+    const int py = oy * e.oy_mul + e.oy_add, px = ox * e.ox_mul + e.ox_add;
+    const size_t opix = ((size_t)nimg * e.oH + py) * e.oW + px;
+    const size_t oplane = (size_t)e.oH * e.oW, opl_pix = (size_t)py * e.oW + px;
+    const size_t so = e.os_hi ? ((size_t)(nimg * e.os_Hp + oy + e.os_pt) * e.os_Wp + ox + e.os_pl) * e.os_pitch + e.os_coff : 0;
+    auto at = [&](const float* b, int cs, int coff, int planar, int c) -> const float* {
+      return planar ? b + ((size_t)nimg * cs + coff + c) * oplane + opl_pix : b + opix * cs + coff + c;
+    };
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = n0 + 8 * j + cl;
+      if (c >= e.Cout) continue;
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if (e.vec2) {
+        // NHWC, even channel strides / offsets, 8-byte aligned operands, Cout even: columns c, c + 1 as one float2
+        if (e.add0) { const float2 a = *reinterpret_cast<const float2*>(e.add0 + opix * e.add0_cs + e.add0_coff + c); v0 += a.x; v1 += a.y; }
+        if (e.scale) { const float2 s = __ldg(reinterpret_cast<const float2*>(e.scale + c)); v0 *= s.x; v1 *= s.y; }
+        if (e.shift) { const float2 s = __ldg(reinterpret_cast<const float2*>(e.shift + c)); v0 += s.x; v1 += s.y; }
+        v0 = act_t<ACT>(v0, e.act); v1 = act_t<ACT>(v1, e.act);
+        if (e.mul1) { const float2 s = __ldg(reinterpret_cast<const float2*>(e.mul1 + c)); v0 *= s.x; v1 *= s.y; }
+        if (e.add1) { const float2 a = *reinterpret_cast<const float2*>(e.add1 + opix * e.add1_cs + e.add1_coff + c); v0 += a.x; v1 += a.y; }
+        if (e.out) *reinterpret_cast<float2*>(e.out + opix * e.out_cs + e.out_coff + c) = make_float2(v0, v1);
+        if (e.os_hi) {                       // producer -> consumer fusion: store the consumer's bf16 hi / mid operands directly
+          if (e.os_scale) {
+            const float2 s = __ldg(reinterpret_cast<const float2*>(e.os_scale + c)), t = __ldg(reinterpret_cast<const float2*>(e.os_shift + c));
+            v0 = fmaf(v0, s.x, t.x); v1 = fmaf(v1, s.y, t.y);
+            if (e.os_relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          }
+          uint32_t hh, mm;
+          split2(v0, v1, hh, mm);
+          *reinterpret_cast<uint32_t*>(e.os_hi + so + c) = hh;
+          *reinterpret_cast<uint32_t*>(e.os_mid + so + c) = mm;
+        }
+      } else {
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const int cc = c + q;
+          if (cc >= e.Cout) break;
+          float x = q ? v1 : v0;
+          if (e.add0) x += *at(e.add0, e.add0_cs, e.add0_coff, e.add0_planar, cc);
+          if (e.scale) x *= __ldg(e.scale + cc);
+          if (e.shift) x += __ldg(e.shift + cc);
+          x = act_t<ACT>(x, e.act);
+          if (e.mul1) x *= __ldg(e.mul1 + cc);
+          if (e.add1) x += *at(e.add1, e.add1_cs, e.add1_coff, e.add1_planar, cc);
+          if (e.out) *const_cast<float*>(at(e.out, e.out_cs, e.out_coff, e.out_planar, cc)) = x;
+          if (e.os_hi) {
+            if (e.os_scale) { x = fmaf(x, __ldg(e.os_scale + cc), __ldg(e.os_shift + cc)); if (e.os_relu) x = fmaxf(x, 0.f); }
+            const __nv_bfloat16 hb = __float2bfloat16_rn(x);
+            const __nv_bfloat16 mb = __float2bfloat16_rn(x - __bfloat162float(hb));
+            e.os_hi[so + cc] = __bfloat16_as_ushort(hb); e.os_mid[so + cc] = __bfloat16_as_ushort(mb);
+          }
+        }
+      }
+    }
+  }
+}

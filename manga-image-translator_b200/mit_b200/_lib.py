@@ -1,7 +1,7 @@
 """ctypes binding of libmitb.so (C ABI declared in include/mitb.h).
 
 The library is built in-tree by ``__graft_entry__.build()`` / ``csrc/Makefile``.  There is no fallback: if the
-shared object is missing, or no Blackwell GPU is visible, loading / context creation raises.
+shared object is missing, or no Hopper (sm_90a) GPU is visible, loading / context creation raises.
 """
 from __future__ import annotations
 
@@ -82,7 +82,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise MitbError(f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                        f"(nvcc, sm_100a). There is no CPU or PyTorch fallback.")
+                        f"(nvcc, sm_90a). There is no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)

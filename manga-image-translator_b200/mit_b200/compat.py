@@ -46,7 +46,7 @@ except Exception:  # noqa: BLE001
         _KEY = ""
 
         def __init__(self):
-            os.makedirs(self.model_dir, exist_ok=True)
+            # nothing is downloaded, so no directory is created (the working directory may be read-only)
             self._key = self._KEY or self.__class__.__name__
             self._loaded = False
 

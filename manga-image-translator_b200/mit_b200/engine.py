@@ -63,7 +63,7 @@ class Engine:
     def __init__(self, device="cuda:0"):
         self.lib = _lib.load()
         if not torch.cuda.is_available():
-            raise MitbError("mit_b200 needs a CUDA (B200, sm_100a) device; there is no CPU fallback")
+            raise MitbError("mit_b200 needs a CUDA (H100, sm_90a) device; there is no CPU fallback")
         self.device = torch.device(device if str(device) != "cuda" else "cuda:0")
         if self.device.type != "cuda":
             raise MitbError(f"mit_b200 runs on CUDA only, got device '{device}'")

@@ -33,7 +33,7 @@ from .host.geometry import warp_record
 
 def _require_cuda(device: str) -> str:
     if not str(device).startswith("cuda"):
-        raise MitbError(f"mit_b200 plugins run on CUDA (B200) only; got device '{device}'. "
+        raise MitbError(f"mit_b200 plugins run on CUDA (H100) only; got device '{device}'. "
                         f"Use the reference classes for CPU execution.")
     return "cuda:0" if device == "cuda" else device
 
@@ -323,7 +323,7 @@ class LamaLargeInpainter(LamaMPEInpainter):
 
 # ----------------------------------------------------------------------------------------------- registration
 def register(mask_refinement: bool = False):
-    """Replace the reference registry entries with the B200 plugins (needs the real manga_translator package).  With
+    """Replace the reference registry entries with the H100 plugins (needs the real manga_translator package).  With
     `mask_refinement=True` also rebind `manga_translator.manga_translator.dispatch_mask_refinement` (manga_translator.py:34, called at
     :1356-1358) to the GPU stage of `mit_b200.mask_refinement` - same signature."""
     if not compat.HAVE_REFERENCE:

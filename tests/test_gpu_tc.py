@@ -1,4 +1,4 @@
-"""The tcgen05 (bf16x3 operand split) convolution against torch CPU fp32 and against the exact-fp32 SIMT kernel.
+"""The wgmma (bf16x3 operand split) convolution against torch CPU fp32 and against the exact-fp32 SIMT kernel.
 Tolerance: the split drops terms of <= ~3*2^-18 relative per product -> 1e-4 of the output scale is a safe bound
 (observed ~1e-6..1e-5); the networks' 1e-3 budget is checked in test_gpu_nets.py with tensor cores on."""
 import pytest
@@ -22,18 +22,18 @@ ACTS = {0: lambda x: x, 1: F.relu, 2: F.gelu, 3: F.silu, 4: torch.sigmoid}
 TC_CASES = [
     # n, cin, h, w, cout, k, stride, pad, mode, act   (all eligible: cin % 8 == 0, cout >= 16)
     (1, 64, 16, 16, 128, 1, 1, 0, "zeros", 0),         # one K block, one tile
-    (1, 128, 20, 24, 256, 1, 1, 0, "zeros", 2),        # BN = 256
+    (1, 128, 20, 24, 256, 1, 1, 0, "zeros", 2),        # two N tiles of 128
     (2, 128, 12, 20, 512, 1, 1, 0, "zeros", 2),        # two N tiles
     (1, 512, 9, 13, 128, 3, 1, 1, "reflect", 1),       # LaMa to_l: K = 4608 (72 K blocks, pipeline wrap-around)
-    (1, 128, 17, 23, 384, 3, 1, 1, "reflect", 0),      # BN = 192 x 2
+    (1, 128, 17, 23, 384, 3, 1, 1, "reflect", 0),      # three N tiles of 128
     (1, 40, 24, 50, 80, 3, 1, 1, "zeros", 0),          # OCR layer1: Cin = 40 (chunks straddle K blocks, not taps)
-    (1, 320, 6, 33, 320, 3, (2, 1), 1, "zeros", 0),    # BN = 160 x 2, stride (2,1)
+    (1, 320, 6, 33, 320, 3, (2, 1), 1, "zeros", 0),    # N padded to 3 tiles of 128, stride (2,1)
     (1, 256, 14, 10, 128, 7, 1, 3, "zeros", 0),        # dense 7x7
     (1, 64, 31, 29, 128, 3, 2, 1, "reflect", 1),       # stride 2, M tail (not a multiple of 128)
     (1, 128, 8, 8, 32, 3, 1, 1, "zeros", 3),           # BN = 32
     (3, 1024, 4, 6, 1024, 2, 2, 0, "zeros", 0),        # downsample conv, 4 N tiles, split-K (16 splits)
-    (1, 1024, 12, 16, 128, 7, 1, 3, "zeros", 0),       # DBNet upconv1-like: M = 192, K = 50176 -> split-K over 74 CTAs
-    (1, 64, 40, 36, 3, 3, 1, 1, "reflect", 4),         # thin output on the tensor cores (BN = 16)
+    (1, 1024, 12, 16, 128, 7, 1, 3, "zeros", 0),       # DBNet upconv1-like: M = 192, K = 50176 -> split-K
+    (1, 64, 40, 36, 3, 3, 1, 1, "reflect", 4),         # thin output on the tensor cores (BN = 32)
     (1, 32, 30, 26, 1, 1, 1, 0, "zeros", 4),           # mask head 1x1 -> 1 channel
     (1, 160, 13, 21, 160, 3, 1, 1, "zeros", 1),        # OCR layer3: Cin = 160 -> per-tap padding to 192 on the TMA path
     (2, 80, 9, 70, 96, 3, 1, 1, "zeros", 0),           # Cin = 80 -> 128, Cout = 96 (BN chosen per launch), batch of 2 patches

@@ -1,240 +1,132 @@
-"""Pins the oracle restatement against the unmodified reference modules imported from /root/reference
-(build container only; skipped on the GPU box where the tree is absent)."""
-import warnings
-
+"""Pins the oracle restatement and the host glue on the unmodified reference modules: what the reference's own code returned on the
+seeded inputs of oracle/ref_pins.py is recorded in tests/golden/reference_pins.{json,npz} (regenerate with `python -m oracle.ref_pins`
+where the reference tree is available); here the oracle / product side is computed and compared with it."""
 import numpy as np
-import pytest
 import torch
 
-from oracle import cases, nets, refload, weights
+from oracle import cases, nets, ref_pins, weights
 
-pytestmark = [pytest.mark.reference,
-              pytest.mark.skipif(not refload.available(), reason="/root/reference not present")]
 torch.set_grad_enabled(False)
 
 
-@pytest.fixture(scope="module")
-def ref():
-    warnings.filterwarnings("ignore")
-    return refload.load()
-
-
-def _check_keys(module, sd):
-    want = {k: tuple(v.shape) for k, v in module.state_dict().items()
-            if "num_batches_tracked" not in k and not k.endswith("pe.pe")}
-    have = {k: tuple(v.shape) for k, v in sd.items()}
-    assert want == have
-
-
-def test_state_dict_specs_match_reference(ref):
-    _check_keys(ref["det"].DBNetConvNext(), weights.dbnet_weights())
-    _check_keys(ref["ocr"].OCR(["x"] * 300, 768), weights.ocr_weights(300))
+def test_state_dict_specs_match_reference():
+    J, _ = ref_pins.load()
+    spec = J["state_dict_specs"]
+    assert spec["dbnet"] == ref_pins.state_dict_spec(weights.dbnet_weights())
+    assert spec["ocr300"] == ref_pins.state_dict_spec(weights.ocr_weights(300))
     for nb in (9, 18):
-        lf = ref["lama"].LamaFourier(build_discriminator=False, use_mpe=nb == 9, large_arch=nb == 18)
-        _check_keys(lf.generator, weights.lama_weights(nb))
-        if nb == 9:
-            _check_keys(lf.mpe, weights.mpe_weights())
-            assert torch.equal(lf.mpe.rel_pos_emb.weight, weights.mpe_weights()["rel_pos_emb.weight"])
+        assert spec[f"lama{nb}"] == ref_pins.state_dict_spec(weights.lama_weights(nb))
+    assert spec["mpe"] == ref_pins.state_dict_spec(weights.mpe_weights())
+    assert spec["mpe_rel_pos_emb"] == ref_pins.digest(weights.mpe_weights()["rel_pos_emb.weight"].numpy())
 
 
-def test_dbnet_rectangular(ref):
+def _sampled(t):
+    flat = t.numpy().reshape(-1)
+    return flat[ref_pins.sample_positions(flat.size)]
+
+
+def test_dbnet_rectangular():
+    J, Z = ref_pins.load()
     sd = weights.dbnet_weights(seed=2)
-    net = ref["det"].DBNetConvNext().eval()
-    net.load_state_dict(sd)
     _, x = cases.dbnet_case(256, 512, seed=21)
-    r_db, r_mask = net(x)
     o_db, o_mask = nets.dbnet_forward(sd, x)
-    assert (r_db - o_db).abs().max() < 1e-4 and (r_mask - o_mask).abs().max() < 1e-5
+    assert list(o_db.shape) == J["dbnet_rect_db_shape"] and list(o_mask.shape) == J["dbnet_rect_mask_shape"]
+    assert np.abs(Z["dbnet_rect_db"] - _sampled(o_db)).max() < 1e-4 and np.abs(Z["dbnet_rect_mask"] - _sampled(o_mask)).max() < 1e-5
 
 
-def test_ocr_widths_and_decode(ref):
+def test_ocr_widths_and_decode():
+    J, Z = ref_pins.load()
     V = 300
     sd = weights.ocr_weights(V, seed=3)
-    ocr = ref["ocr"].OCR(weights.synthetic_dictionary(V), 768).eval()
-    ocr.load_state_dict(sd, strict=False)
     for wp in (143, 200, 331):
+        rec = J["ocr_widths"][str(wp)]
         _, x = cases.ocr_case(3, wp, seed=wp)
-        rl, rc = ocr(x)
         ol, oc = nets.ocr_forward(sd, x)
-        assert (rl - ol).abs().max() < 1e-4 and (rc - oc).abs().max() < 1e-5
+        assert list(ol.shape) == rec["logits_shape"]
+        assert np.abs(Z[f"ocr_logits_{wp}"] - _sampled(ol)).max() < 1e-4 and np.abs(Z[f"ocr_colors_{wp}"] - oc.numpy()).max() < 1e-5
         idx, lp, col = nets.ocr_top1(sd, x)
-        ref_dec = ocr.decode(x, [0] * 3, 0)
         mine = nets.ctc_greedy(idx.numpy(), lp.numpy(), col.numpy())
-        top2 = rl.topk(2, dim=-1).values
-        if (top2[..., 0] - top2[..., 1]).min() > 1e-3:
-            assert [[int(c[0]) for c in l] for l in ref_dec] == [[c[0] for c in l] for l in mine]
+        if rec["margin_ok"]:
+            assert rec["decode"] == [[c[0] for c in l] for l in mine]
 
 
-def test_lama_mpe_tables_random_masks(ref):
-    lf = ref["lama"].LamaFourier(build_discriminator=False, use_mpe=True)
-    rng = np.random.default_rng(5)
-    for (h, w) in ((256, 256), (200, 312), (64, 48)):
-        m = np.zeros((h, w), np.float32)
-        for _ in range(4):
-            y, x = rng.integers(0, h - 8), rng.integers(0, w - 8)
-            m[y:y + rng.integers(4, h // 2), x:x + rng.integers(4, w // 2)] = 1
-        rel, _, direct = lf.load_masked_position_encoding(m)
+def test_lama_mpe_tables_random_masks():
+    J, _ = ref_pins.load()
+    masks = ref_pins.mpe_masks()
+    assert len(masks) == len(J["mpe_tables"])
+    for m, want in zip(masks, J["mpe_tables"]):
         orel, odirect = nets.mpe_tables(m)
-        assert np.array_equal(rel, orel) and np.array_equal(direct, odirect)
-    # all-hole and no-hole masks terminate (the reference guards the infinite loop, :778)
-    for m in (np.zeros((64, 64), np.float32), np.ones((64, 64), np.float32)):
-        rel, _, direct = lf.load_masked_position_encoding(m)
-        orel, odirect = nets.mpe_tables(m)
-        assert np.array_equal(rel, orel) and np.array_equal(direct, odirect)
+        assert ref_pins.digest(orel) == want["rel"] and ref_pins.digest(odirect) == want["direct"]
 
 
-def test_lama_odd_spectrum_sizes(ref):
+def test_lama_odd_spectrum_sizes():
+    _, Z = ref_pins.load()
     sd, msd = weights.lama_weights(9, seed=4), weights.mpe_weights(seed=4)
-    lf = ref["lama"].LamaFourier(build_discriminator=False, use_mpe=True)
-    lf.generator.load_state_dict(sd)
-    lf.mpe.load_state_dict(msd)
-    lf.eval()
     img, mask = cases.lama_case(88, 120, seed=41)   # bottleneck 11x15: odd FFT lengths
-    r = lf(img.clone(), mask)
     rel, direct = nets.mpe_tables(mask[0, 0].numpy())
     o = nets.lama_forward(sd, msd, img, mask, torch.from_numpy(rel)[None], torch.from_numpy(direct)[None])
-    assert (r - o).abs().max() < 2e-5
+    assert np.abs(Z["lama_odd"] - o.numpy()).max() < 2e-5
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # The three `_infer` glue paths: oracle/pipeline_ref.py (what the GPU plugin tests compare the product with) against the reference's own
-# `_infer` methods, executed unmodified on the CPU with a duck-typed `self` (constructing the plugin classes would need model
-# directories) and the absent third-party libraries bound to the repo's restatements (pyclipper -> Clipper 6.4.2 restatement, shapely ->
-# geometry restatements).  Closes the loop: reference `_infer` == pipeline_ref here, plugin == pipeline_ref on the GPU.
-def _bind_third_party(ref):
-    import importlib
-    import sys
-    from mit_b200.host import det_post, geometry
-    G = importlib.import_module("manga_translator.utils.generic")
-    du = importlib.import_module("manga_translator.detection.default_utils.dbnet_utils")
-
-    class _Offset:
-        def AddPath(self, box, jt, et):
-            self.box = box
-
-        def Execute(self, d):
-            return [det_post.clipper_offset_round(self.box, d)]
-
-    class Polygon:
-        def __init__(self, pts):
-            self.p = np.asarray(pts, dtype=np.float64).reshape(-1, 2)
-            self.area, self.length = geometry.polygon_area(self.p), geometry.polygon_perimeter(self.p)
-
-        @property
-        def convex_hull(self):
-            return Polygon(geometry._hull(self.p))
-
-        def distance(self, other):
-            return geometry.polygon_distance(self.p, other.p)
-
-    saved = (du.pyclipper, du.Polygon, G.Polygon, G.MultiPoint)
-    du.pyclipper = type("pc", (), dict(PyclipperOffset=_Offset, JT_ROUND=1, ET_CLOSEDPOLYGON=2))
-    du.Polygon = G.Polygon = G.MultiPoint = Polygon
-
-    def restore():
-        du.pyclipper, du.Polygon, G.Polygon, G.MultiPoint = saved
-    return restore
-
-
-def test_detector_infer_glue_equals_reference_code(ref):
-    import asyncio
-    import logging
-    import types
-    from mit_b200 import synth
+# `_infer` methods, recorded from an unmodified run on the CPU with a duck-typed `self` and the absent third-party libraries bound to
+# the repo's restatements (pyclipper -> Clipper 6.4.2 restatement, shapely -> geometry restatements).  Closes the loop: reference
+# `_infer` == pipeline_ref here, plugin == pipeline_ref on the GPU.
+def test_detector_infer_glue_equals_reference_code():
     from oracle import pipeline_ref
-    det = ref["det"]
-    sd = {k: v.clone() for k, v in weights.dbnet_weights().items()}
-    sd["conv_db.binarize.4.bias"] -= 1.0
-    net = det.DBNetConvNext().eval()
-    net.load_state_dict(sd)
-    det.MODEL = net
-    me = types.SimpleNamespace(device="cpu", logger=logging.getLogger("ref-det"), model=net)
-    restore = _bind_third_party(ref)
-    try:
-        for page, detect_size in ((synth.make_page(5, 512, 384, 6)[0], 512), (synth.make_page(4, 384, 384, 5)[0], 512)):   # pad path; upscale path
-            r_lines, r_mask, _ = asyncio.run(det.DBConvNextDetector._infer(me, page, detect_size, 0.5, 0.6, 2.3))
-            o_lines, o_mask, _, _ = pipeline_ref.detector_infer(sd, page, detect_size, 0.5, 0.6, 2.3)
-            assert len(r_lines) == len(o_lines) and len(r_lines) > 3
-            for a, b in zip(r_lines, o_lines):
-                assert np.array_equal(a.pts, b.pts) and a.prob == b.prob and a.direction == b.direction
-            assert r_mask.dtype == np.uint8 and np.array_equal(r_mask, o_mask)
-    finally:
-        restore()
+    J, _ = ref_pins.load()
+    sd = ref_pins.detector_glue_weights()
+    for (page, detect_size), want in zip(ref_pins.detector_glue_pages(), J["detector_glue"]):
+        o_lines, o_mask, _, _ = pipeline_ref.detector_infer(sd, page, detect_size, 0.5, 0.6, 2.3)
+        assert len(want["lines"]) == len(o_lines) and len(o_lines) > 3
+        for a, b in zip(want["lines"], o_lines):
+            assert np.array_equal(np.array(a["pts"]), b.pts) and a["prob"] == b.prob and a["direction"] == b.direction
+        assert want["mask_dtype"] == "uint8" and ref_pins.digest(o_mask) == want["mask"]
 
 
-def test_ocr_infer_glue_equals_reference_code(ref):
-    import asyncio
-    import logging
-    import sys
-    import types
+def test_ocr_infer_glue_equals_reference_code():
     from mit_b200 import synth
     from mit_b200.host import geometry
     from oracle import pipeline_ref
+    J, _ = ref_pins.load()
     V = cases.OCR_VOCAB_SMALL
     dictionary = weights.synthetic_dictionary(V)
     sd = weights.ocr_weights(V)
-    model = ref["ocr"].OCR(dictionary, 768).eval()
-    model.load_state_dict(sd, strict=False)
-    common = sys.modules["manga_translator.ocr.common"]
     page, boxes, _ = synth.make_page(3, 512, 384, 6)
-    U = ref["utils"]
-    restore = _bind_third_party(ref)
-    try:
-        me = types.SimpleNamespace(device="cpu", use_gpu=False, logger=logging.getLogger("ref-ocr"), model=model)
-        me._generate_text_direction = lambda bboxes: common.CommonOCR._generate_text_direction(me, bboxes)
-        r_quads = [U.Quadrilateral(b.copy(), "", 1.0) for b in boxes]
-        cfg = types.SimpleNamespace(ignore_bubble=0, prob=0.0)
-        r_out = asyncio.run(ref["ocr"].Model48pxCTCOCR._infer(me, page, r_quads, cfg, False))
-        o_out = pipeline_ref.ocr_infer(sd, dictionary, page, [geometry.Quadrilateral(b.copy(), "", 1.0) for b in boxes], 0.0)
-        assert len(r_out) == len(o_out) >= 4
-        for a, b in zip(r_out, o_out):
-            assert np.array_equal(a.pts, b.pts) and a.text == b.text and len(a.text) > 0
-            assert abs(a.prob - b.prob) < 1e-4 * max(a.prob, 1e-30)            # the two fp32 network evaluations differ by ~1e-5 in log-probability
-            assert (a.fg_r, a.fg_g, a.fg_b, a.bg_r, a.bg_g, a.bg_b) == (b.fg_r, b.fg_g, b.fg_b, b.bg_r, b.bg_g, b.bg_b)
-    finally:
-        restore()
+    r_out = J["ocr_glue"]
+    o_out = pipeline_ref.ocr_infer(sd, dictionary, page, [geometry.Quadrilateral(b.copy(), "", 1.0) for b in boxes], 0.0)
+    assert len(r_out) == len(o_out) >= 4
+    for a, b in zip(r_out, o_out):
+        assert np.array_equal(np.array(a["pts"]), b.pts) and a["text"] == b.text and len(a["text"]) > 0
+        assert abs(a["prob"] - b.prob) < 1e-4 * max(a["prob"], 1e-30)            # the two fp32 network evaluations differ by ~1e-5 in log-probability
+        assert tuple(a["colors"]) == (b.fg_r, b.fg_g, b.fg_b, b.bg_r, b.bg_g, b.bg_b)
 
 
-def test_inpainter_infer_glue_equals_reference_code(ref):
-    import asyncio
-    import logging
-    import types
-    from mit_b200 import synth
+def test_inpainter_infer_glue_equals_reference_code():
     from oracle import pipeline_ref
-    lama = ref["lama"]
+    _, Z = ref_pins.load()
     sd, msd = weights.lama_weights(9), weights.mpe_weights()
-    lf = lama.LamaFourier(build_discriminator=False, use_mpe=True)
-    lf.generator.load_state_dict(sd)
-    lf.mpe.load_state_dict(msd)
-    lf.eval()
-    me = types.SimpleNamespace(device="cpu", logger=logging.getLogger("ref-inp"), model=lf)
-    rng = np.random.default_rng(6)
-    page = rng.integers(0, 256, (200, 152, 3), dtype=np.uint8)
-    mask = np.zeros((200, 152), np.uint8)
-    mask[20:50, 10:120] = 255
-    mask[120:180, 60:90] = 255
-    mask[100:104, 5:40] = 130
-    mask[10, 10] = 127                                            # the 127 / 128 threshold quirk (SURVEY I2)
-    for size in (1024, 128):                                      # no resize; keep-aspect resize + back
-        r = asyncio.run(lama.LamaMPEInpainter._infer(me, page.copy(), mask.copy(), types.SimpleNamespace(inpainting_precision="fp32"), size, False))
+    page, mask, sizes = ref_pins.inpainter_glue_case()
+    for size in sizes:                                            # no resize; keep-aspect resize + back
+        r = Z[f"inpainter_glue_{size}"]
         o, _ = pipeline_ref.lama_infer(sd, msd, page.copy(), mask.copy(), size)
         assert r.dtype == o.dtype == np.uint8 and r.shape == page.shape
         d = np.abs(r.astype(int) - o.astype(int))
         assert d.max() <= 1 and (d > 0).mean() < 1e-3, (int(d.max()), float((d > 0).mean()))     # x*255 truncation of fp32 values 2e-5 apart
 
 
-def test_common_detector_detect_equals_reference_code(ref):
+def test_common_detector_detect_equals_reference_code():
     """D12: the stand-in `CommonDetector.detect` of mit_b200.compat (border for small pages, rotation, inversion, gamma correction,
     auto-rotation; used when the reference package cannot be imported) against the reference's own `detection/common.py` code, both
-    wrapped around the same stub `_detect`: identical text lines, raw mask and mask for every combination of the switches."""
+    wrapped around the same stub `_detect` (oracle/ref_pins.py): identical images handed to `_detect`, text lines, raw mask and mask
+    for every combination of the switches."""
     import asyncio
-    import importlib
-    import itertools
     import importlib.util
     import sys
     from mit_b200 import compat as _compat_loaded
     from mit_b200.host import geometry
-    rc = importlib.import_module("manga_translator.detection.common")
+    J, _ = ref_pins.load()
     # a second copy of mit_b200/compat.py imported while `manga_translator` is hidden: that is the stand-in the GPU box gets
     hidden = {k: sys.modules.pop(k) for k in list(sys.modules) if k == "manga_translator" or k.startswith("manga_translator.")}
     sys.modules["manga_translator"] = None                       # makes `import manga_translator...` raise ImportError
@@ -247,29 +139,9 @@ def test_common_detector_detect_equals_reference_code(ref):
         del sys.modules["manga_translator"]
         sys.modules.update(hidden)
     assert not compat.HAVE_REFERENCE
-    U = ref["utils"]
-    restore = _bind_third_party(ref)
-
-    def stub(quad_cls):
-        async def _detect(self, image, detect_size, text_threshold, box_threshold, unclip_ratio, verbose=False):
-            self.seen.append(image.copy())
-            h, w = image.shape[:2]
-            rng = np.random.default_rng(h * 7919 + w)
-            lines = []
-            for _ in range(6):
-                x0, y0 = int(rng.integers(0, w - 40)), int(rng.integers(0, h - 40))
-                bw, bh = int(rng.integers(12, 120)), int(rng.integers(8, 60))
-                lines.append(quad_cls(np.array([[x0, y0], [x0 + bw, y0], [x0 + bw, y0 + bh], [x0, y0 + bh]]), "", 0.9))
-            lines.append(quad_cls(np.array([[5, 5], [6, 5], [6, 6], [5, 6]]), "", 0.5))          # area 1: filtered
-            raw = (rng.random((h, w)) * 255).astype(np.uint8)
-            return lines, raw, (rng.random((h, w)) > 0.5).astype(np.uint8) * 255
-        return _detect
-
-    class RefDet(rc.CommonDetector):
-        _detect = stub(U.Quadrilateral)
 
     class OurDet(compat.OfflineDetector):
-        _detect = stub(geometry.Quadrilateral)
+        _detect = ref_pins.detector_stub(geometry.Quadrilateral)
 
         async def _load(self, device):
             pass
@@ -280,17 +152,12 @@ def test_common_detector_detect_equals_reference_code(ref):
         async def _infer(self, *a, **k):
             raise AssertionError("not used: `_detect` is stubbed")
 
-    try:
-        rng = np.random.default_rng(2)
-        for (h, w) in ((300, 200), (520, 450), (380, 700)):
-            img = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
-            for invert, gamma, rotate, auto in itertools.product((False, True), repeat=4):
-                r, o = RefDet(), OurDet()
-                r.seen, o.seen = [], []
-                rt, rraw, rmask = asyncio.run(r.detect(img.copy(), 1024, 0.5, 0.7, 2.3, invert, gamma, rotate, auto))
-                ot, oraw, omask = asyncio.run(o.detect(img.copy(), 1024, 0.5, 0.7, 2.3, invert, gamma, rotate, auto))
-                assert len(r.seen) == len(o.seen) and all(np.array_equal(a, b) for a, b in zip(r.seen, o.seen)), (h, w, invert, gamma, rotate, auto)
-                assert len(rt) == len(ot) and all(np.array_equal(a.pts, b.pts) for a, b in zip(rt, ot))
-                assert np.array_equal(rraw, oraw) and np.array_equal(rmask, omask)
-    finally:
-        restore()
+    cases_ = ref_pins.common_detector_cases()
+    assert len(cases_) == len(J["common_detector"])
+    for (h, w, img, sw), want in zip(cases_, J["common_detector"]):
+        o = OurDet()
+        o.seen = []
+        ot, oraw, omask = asyncio.run(o.detect(img.copy(), 1024, 0.5, 0.7, 2.3, *sw))
+        assert want["seen"] == [ref_pins.digest(a) for a in o.seen], (h, w, sw)
+        assert want["lines"] == (ref_pins.digest(np.stack([b.pts for b in ot])) if ot else None)
+        assert want["raw"] == ref_pins.digest(oraw) and want["mask"] == ref_pins.digest(omask)
