@@ -7,12 +7,12 @@
 //   warp 8      producer: per K block (= 64 channels of one tap) four TMA loads - the activation box {64 ch, bw, bh} of the
 //               hi and mid tensors at the tap-shifted pixel coordinates (zero padding = TMA out-of-bounds fill) and the
 //               weight boxes {64 k, BN} - all landing in the K-major SWIZZLE_128B layout, completing on the stage's "full"
-//               mbarrier (expect_tx); a ring of 3..6 stages;
-//   warps 0-7   two consumer warpgroups, 64 rows of the 128-row tile each: 12 wgmma per K block (bf16x3: Ah*Bh + Ah*Bm + Am*Bh,
-//               fp32 accumulators in registers), the stage is released on its "empty" mbarrier once the wgmma that read it
-//               retired (one K block of wgmma stays in flight); then the epilogue straight from the accumulator registers
-//               ((+add0)*scale+shift -> act -> *mul1 -> +add1 -> fp32 stores and / or split operands, tc_common.cuh) while the
-//               producer already streams the next tile's operands.
+//               mbarrier (expect_tx); a ring of 3..6 stages; warps 9-11 of its warpgroup exit once they gave up their registers;
+//   warps 0-7   two consumer warpgroups in ping-pong: each owns whole 128-row tiles, alternately, and issues 24 wgmma per K
+//               block (two 64-row halves, bf16x3: Ah*Bh + Ah*Bm + Am*Bh, fp32 accumulators in registers); the stage is released
+//               on its "empty" mbarrier once the wgmma that read it retired (one K block of wgmma stays in flight); then the
+//               epilogue straight from the accumulator registers ((+add0)*scale+shift -> act -> *mul1 -> +add1 -> fp32 stores
+//               and / or split operands, tc_common.cuh) while the other warpgroup's main loop runs on the tensor core.
 // Operand fusion (ConvOp::in_sv / out_sv / seg2): a producer's epilogue can store its result directly as the consumer's bf16
 // hi/mid operand tensor (SplitView, optionally with a reflect halo and the consumer's BN+ReLU prologue applied), so the split
 // pass disappears; and a second K segment with its own tensor maps lets two convolutions of different inputs accumulate into one
@@ -31,8 +31,11 @@ namespace mitb {
 namespace {
 
 constexpr int TC_BM = 128, TC_BK = 64;
-constexpr int TM_CWARPS = 8;                         // two consumer warpgroups
-constexpr int TM_THREADS = TM_CWARPS * 32 + 32;      // + the producer warp
+constexpr int TM_WG_WARPS = 4;
+constexpr int TM_THREADS = 3 * TM_WG_WARPS * 32;     // two consumer warpgroups + the producer warpgroup
+// Register split: 2 x 128 x 232 + 128 x 40 <= 64 K.  Any 3 warps of one SM sub-partition are capped at 168 registers each
+// otherwise, too few for a warpgroup's 128 x 128 accumulator (128 registers) next to its epilogue.
+constexpr int TM_CONSUMER_REGS = 232, TM_PRODUCER_REGS = 40;
 
 #include "tc_common.cuh"
 
@@ -50,6 +53,21 @@ struct TmaParams {
   const uint8_t* tile_need;                                   // per 128-row M tile: 0 = skip (ConvOp::need_px reduced over the tile), null: all
   EpiParams e;
 };
+
+// Phase timing (build with EXTRA=-DMITB_CONV_PHASES, read by tools/conv_phases.py): clock64 sums over all consumer warpgroups
+// of a launch for [0] the wait on a tile's first full barrier, [1] the main loop, [2] wgmma_wait<0>, [3] the epilogue; [4] counts
+// processed tiles.  The default build contains none of it.
+#ifdef MITB_CONV_PHASES
+__device__ unsigned long long g_conv_phases[5];
+#define PHASE_CLOCK(v) v = clock64()
+#else
+#define PHASE_CLOCK(v)
+#endif
+
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // expect_tx + the four operand boxes of one K block, issued by one elected lane of a converged warp
 __device__ __forceinline__ void tma_kblock(uint32_t bar, uint32_t bytes, uint32_t a_hi, uint32_t a_mid, uint32_t b_hi, uint32_t b_mid,
@@ -89,7 +107,7 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
   const int total_tiles = mt * nt;
 
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TM_CWARPS); }
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TM_WG_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -105,36 +123,65 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
   // output sparsity: every role walks the same tile sequence and skips the same tiles
   auto needed = [&](int t) -> bool { return !p.tile_need || p.tile_need[t / nt] != 0; };
 
-  if (warp < TM_CWARPS) {
-    // =========================== consumers: wgmma main loop + epilogue ===========================
+  if (warp < 2 * TM_WG_WARPS) {
+    // =========================== consumers: ping-pong over whole tiles ===========================
+    // Warpgroup wg takes the processed tiles j with j % 2 == wg and runs main loop and epilogue of the full 128 x BN tile.  Two
+    // named barriers hand the tensor core from one warpgroup to the other once a main loop has issued its last K block, so the
+    // epilogue of one tile runs while the other warpgroup's main loop keeps the tensor core busy.
+    setmaxnreg_inc<TM_CONSUMER_REGS>();
     const int wg = warp >> 2;
     const int HoWo = p.Ho * p.Wo;
+    const int row = (warp & 3) * 16 + (lane >> 2);
     int s = 0; uint32_t ph = 0;
+    int j = 0;                                           // tiles processed by this CTA so far, both warpgroups
+    if (wg == 1) named_bar_arrive(1, 2 * TM_WG_WARPS * 32);   // warpgroup 0 takes the first turn
+#ifdef MITB_CONV_PHASES
+    long long c0 = 0, c1 = 0, c2 = 0, c3 = 0, c4 = 0, sum[4] = {0, 0, 0, 0}, ntl = 0;
+#endif
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       if (!needed(t)) continue;
+      if ((j++ & 1) != wg) {                             // the other warpgroup's tile: skip its stages of the ring
+        const int q = s + nkb;
+        ph ^= (uint32_t)((q / S) & 1);
+        s = q % S;
+        continue;
+      }
       int nimg_t, oy0, ox0, n0;
       decode(t, nimg_t, oy0, ox0, n0);
-      float acc[BN / 2];
+      float acc0[BN / 2], acc1[BN / 2];                  // rows 0-63 and 64-127 of the tile
       int prev = -1;
+      named_bar_sync(1 + wg, 2 * TM_WG_WARPS * 32);       // this warpgroup's turn on the tensor core
+      PHASE_CLOCK(c0);
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(full_bar(s), ph);
-        const uint32_t a_hi = smem_base + (uint32_t)s * stage_bytes + (uint32_t)wg * (64u * 128u), a_mid = a_hi + a_bytes;
-        const uint32_t b_hi = smem_base + (uint32_t)s * stage_bytes + 2 * a_bytes, b_mid = b_hi + b_bytes;
-        fence_acc(acc);
+#ifdef MITB_CONV_PHASES
+        if (kb == 0) c1 = clock64();
+#endif
+        const uint32_t a_hi = smem_base + (uint32_t)s * stage_bytes, a_mid = a_hi + a_bytes;
+        const uint32_t b_hi = a_mid + a_bytes, b_mid = b_hi + b_bytes;
+        const uint64_t dbh = make_desc_sw128(b_hi), dbm = make_desc_sw128(b_mid);
+        fence_acc(acc0);
+        fence_acc(acc1);
         wgmma_fence();
-        wgmma_kblock_x3<BN>(acc, make_desc_sw128(a_hi), make_desc_sw128(a_mid), make_desc_sw128(b_hi), make_desc_sw128(b_mid), kb == 0);
+        wgmma_kblock_x3<BN>(acc0, make_desc_sw128(a_hi), make_desc_sw128(a_mid), dbh, dbm, kb == 0);
+        wgmma_kblock_x3<BN>(acc1, make_desc_sw128(a_hi + 64u * 128u), make_desc_sw128(a_mid + 64u * 128u), dbh, dbm, kb == 0);
         wgmma_commit();
         wgmma_wait<1>();                                 // the previous K block's wgmma retired -> its stage is free
-        fence_acc(acc);
+        fence_acc(acc0);
+        fence_acc(acc1);
         if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
         prev = s;
         if (++s == S) { s = 0; ph ^= 1u; }
       }
+      named_bar_arrive(1 + (wg ^ 1), 2 * TM_WG_WARPS * 32);   // the other warpgroup's turn
+      PHASE_CLOCK(c2);
       wgmma_wait<0>();
-      fence_acc(acc);
+      fence_acc(acc0);
+      fence_acc(acc1);
+      PHASE_CLOCK(c3);
       __syncwarp();
       if (lane == 0) mbar_arrive(empty_bar(prev));
-      epilogue_tile<ACT, BN>(p.e, acc, wg * 64 + (warp & 3) * 16 + (lane >> 2), n0, 0, [&](int r, int& nimg, int& oy, int& ox) -> bool {
+      auto rowpix = [&](int r, int& nimg, int& oy, int& ox) -> bool {
         if (p.lin) {
           const int m = ox0 + r;
           if (m >= p.M || nimg_t >= p.N) return false;
@@ -144,10 +191,26 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
         }
         nimg = nimg_t; oy = oy0 + (r >> p.bw_log2); ox = ox0 + (r & (bw - 1));
         return oy < p.Ho && ox < p.Wo && nimg < p.N;
-      });
+      };
+      epilogue_tile<ACT, BN>(p.e, acc0, row, n0, 0, rowpix);
+      epilogue_tile<ACT, BN>(p.e, acc1, 64 + row, n0, 0, rowpix);
+#ifdef MITB_CONV_PHASES
+      c4 = clock64();
+      sum[0] += c1 - c0; sum[1] += c2 - c1; sum[2] += c3 - c2; sum[3] += c4 - c3; ++ntl;
+#endif
     }
+    // the turn opened after the last tile is taken by the warpgroup it was opened for, so both barriers end balanced
+    if ((j & 1) == wg) named_bar_sync(1 + wg, 2 * TM_WG_WARPS * 32);
+#ifdef MITB_CONV_PHASES
+    if ((tid & 127) == 0) {
+      for (int i = 0; i < 4; ++i) atomicAdd(&g_conv_phases[i], (unsigned long long)sum[i]);
+      atomicAdd(&g_conv_phases[4], (unsigned long long)ntl);
+    }
+#endif
   } else {
-    // =========================== producer: four TMA boxes per K block (whole warp loops, one elected lane issues) =====
+    // =========================== producer warpgroup: its first warp issues four TMA boxes per K block =============
+    setmaxnreg_dec<TM_PRODUCER_REGS>();
+    if (warp != 2 * TM_WG_WARPS) return;
     int s = 0; uint32_t ph = 1;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       if (!needed(t)) continue;
@@ -337,15 +400,17 @@ void make_w_tmap(CUtensorMap* m, const uint16_t* base, int kdim, int rows, int b
   MITB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for weights [%d x %d] box %d", (int)r, rows, kdim, bn);
 }
 
-// N tile width: minimise waves x tile time.  Tile time = K blocks x max(tensor floor, operand bytes over the SM's share of L2
-// bandwidth) + epilogue + a fixed cost; candidates split Cout into j equal tiles rounded up to 32 (the wgmma widths instantiated,
-// at most 128).  Tensor floor: 3 x 128 x bn x 64 bf16 MACs per K block at the H100 SXM data-sheet dense bf16 rate (~2048 MAC per
-// clock per SM) = 12 bn cycles.  The epilogue runs after the main loop on the same warps (accumulators in registers), so the
-// two add.  The L2 share (42 B/clk) and the epilogue cycles per column are estimates, not measurements; MITB_CM=
-// "mode,epi_gelu,epi,fix" overrides the constants (mode 1: max instead of sum; tools/cost_model_sweep.py).
+// N tile width: minimise waves x tile time.  Main loop = K blocks x max(tensor floor, operand bytes over the SM's share of L2
+// bandwidth); candidates split Cout into j equal tiles rounded up to 32 (the wgmma widths instantiated, at most 128).  Tensor
+// floor: 3 x 128 x bn x 64 bf16 MACs per K block at the H100 SXM data-sheet dense bf16 rate (~2048 MAC per clock per SM) =
+// 12 bn cycles (measured with tools/conv_phases.py: 1490-1660 clk per K block at bn = 128 on L2-resident layers).  The two
+// consumer warpgroups alternate whole tiles and one warpgroup's epilogue overlaps the other's main loop, so a CTA finishes two
+// tiles per max(2 main, main + epilogue): tile time = max(main, (main + epilogue) / 2) + a fixed cost (mode 1; mode 0 is the
+// sum, for a schedule without overlap).  The epilogue cycles per column are measured (tools/conv_phases.py), the L2 share (42 B/clk)
+// is an estimate; MITB_CM="mode,epi_gelu,epi,fix" overrides the constants (tools/cost_model_sweep.py).
 struct CostModel { int mode; double epi_gelu, epi, fix; };
 const CostModel& cost_model() {
-  static CostModel cm = {0, 40.0, 40.0, 600.0};
+  static CostModel cm = {1, 450.0, 450.0, 600.0};
   static bool init = false;
   if (!init) {
     init = true;
@@ -367,7 +432,8 @@ int choose_bn(int Cout, long mtiles, int nkb, int sms, bool gelu) {
     const long waves = (mtiles * nt + sms - 1) / sms;
     const double mma = 12.0 * bn, l2 = (32768.0 + 256.0 * bn) / 42.0;
     const double main_loop = nkb * (mma > l2 ? mma : l2), epi = (gelu ? cm.epi_gelu : cm.epi) * bn;
-    const double tile = (cm.mode == 1 ? (main_loop > epi ? main_loop : epi) : main_loop + epi) + cm.fix;
+    const double overlap = (main_loop + epi) / 2;
+    const double tile = (cm.mode == 1 ? (main_loop > overlap ? main_loop : overlap) : main_loop + epi) + cm.fix;
     const double cost = waves * tile;
     if (cost < best * 0.999) { best = cost; best_bn = bn; }
   }
@@ -637,6 +703,18 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
   count_launch();
   g_key_epoch = g_launch_epoch;
   CUDA_OK(cudaGetLastError());
+#ifdef MITB_CONV_PHASES
+  {
+    unsigned long long ph[5];
+    CUDA_OK(cudaStreamSynchronize(st));
+    CUDA_OK(cudaMemcpyFromSymbol(ph, g_conv_phases, sizeof(ph)));
+    const unsigned long long zero[5] = {0, 0, 0, 0, 0};
+    CUDA_OK(cudaMemcpyToSymbol(g_conv_phases, zero, sizeof(zero)));
+    const int K = op.ntaps * C + (two ? op.seg2.ntaps * op.seg2.C : 0);      // the GEMM shape tools/layer_times.py reports
+    fprintf(stderr, "mitb_conv_phases M %d K %d N %d BN %d nkb %d ctas %d tiles %llu first_wait %llu main %llu wgmma_wait %llu epilogue %llu\n",
+            N * op.Ho * op.Wo, K, op.out.C, BN, p.nkb, grid, ph[4], ph[0], ph[1], ph[2], ph[3]);
+  }
+#endif
 }
 
 }  // namespace mitb

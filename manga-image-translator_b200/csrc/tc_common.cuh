@@ -244,86 +244,146 @@ template <int ACT, int BN, class RowPix>
 __device__ __forceinline__ void epilogue_tile(const EpiParams& e, const float (&acc)[BN / 2], int row0, int n0, int z, RowPix rowpix) {
   const int lane = threadIdx.x & 31;
   const int cl = 2 * (lane & 3);
+  if (e.stat_max || e.partial) {
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    int nimg = 0, oy = 0, ox = 0;
-    const bool ok = rowpix(row0 + 8 * h, nimg, oy, ox);
-    if (e.stat_max) {
-      // online (max, first argmax, sum exp) per column half of the N tile over this thread's columns, then over the 4 lanes of
-      // the row (model_48px_ctc.py:460-461); the logits never leave the registers
-      constexpr int kHalf = ((BN / 16 + 1) / 2) * 16;
-      float bm[2] = {-INFINITY, -INFINITY}, bs[2] = {0.f, 0.f}; int bi[2] = {0x7fffffff, 0x7fffffff};
+    for (int h = 0; h < 2; ++h) {
+      int nimg = 0, oy = 0, ox = 0;
+      const bool ok = rowpix(row0 + 8 * h, nimg, oy, ox);
+      if (e.stat_max) {
+        // online (max, first argmax, sum exp) per column half of the N tile over this thread's columns, then over the 4 lanes of
+        // the row (model_48px_ctc.py:460-461); the logits never leave the registers
+        constexpr int kHalf = ((BN / 16 + 1) / 2) * 16;
+        float bm[2] = {-INFINITY, -INFINITY}, bs[2] = {0.f, 0.f}; int bi[2] = {0x7fffffff, 0x7fffffff};
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
+        for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          const int cc = 8 * j + cl + q, c = n0 + cc, hf = cc < kHalf ? 0 : 1;
-          if (c < e.Cout) {
-            const float x = acc[4 * j + 2 * h + q] + (e.shift ? __ldg(e.shift + c) : 0.f);
-            if (x > bm[hf]) { bs[hf] = bs[hf] * expf(bm[hf] - x) + 1.f; bm[hf] = x; bi[hf] = c; }
-            else bs[hf] += expf(x - bm[hf]);
+          for (int q = 0; q < 2; ++q) {
+            const int cc = 8 * j + cl + q, c = n0 + cc, hf = cc < kHalf ? 0 : 1;
+            if (c < e.Cout) {
+              const float x = acc[4 * j + 2 * h + q] + (e.shift ? __ldg(e.shift + c) : 0.f);
+              if (x > bm[hf]) { bs[hf] = bs[hf] * expf(bm[hf] - x) + 1.f; bm[hf] = x; bi[hf] = c; }
+              else bs[hf] += expf(x - bm[hf]);
+            }
           }
         }
-      }
 #pragma unroll
-      for (int hf = 0; hf < 2; ++hf) {
+        for (int hf = 0; hf < 2; ++hf) {
 #pragma unroll
-        for (int o = 1; o <= 2; o <<= 1)
-          stat_merge(bm[hf], bs[hf], bi[hf], __shfl_xor_sync(0xffffffffu, bm[hf], o), __shfl_xor_sync(0xffffffffu, bs[hf], o),
-                     __shfl_xor_sync(0xffffffffu, bi[hf], o));
-        if (ok && (lane & 3) == 0) {
-          const size_t o = (((size_t)nimg * e.Ho + oy) * e.Wo + ox) * e.stat_ld + (n0 / BN) * 2 + hf;
-          e.stat_max[o] = bm[hf]; e.stat_sum[o] = bs[hf]; e.stat_idx[o] = bi[hf];
+          for (int o = 1; o <= 2; o <<= 1)
+            stat_merge(bm[hf], bs[hf], bi[hf], __shfl_xor_sync(0xffffffffu, bm[hf], o), __shfl_xor_sync(0xffffffffu, bs[hf], o),
+                       __shfl_xor_sync(0xffffffffu, bi[hf], o));
+          if (ok && (lane & 3) == 0) {
+            const size_t o = (((size_t)nimg * e.Ho + oy) * e.Wo + ox) * e.stat_ld + (n0 / BN) * 2 + hf;
+            e.stat_max[o] = bm[hf]; e.stat_sum[o] = bs[hf]; e.stat_idx[o] = bi[hf];
+          }
         }
+        continue;
       }
-      continue;
-    }
-    if (!ok) continue;
-    if (e.partial) {
+      if (!ok) continue;
       // split-K partial: raw accumulators to partial[z][m][npad]
       float* dst = e.partial + ((size_t)z * e.M + ((size_t)nimg * e.Ho + oy) * e.Wo + ox) * e.npad + n0 + cl;
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-      continue;
     }
-    const int py = oy * e.oy_mul + e.oy_add, px = ox * e.ox_mul + e.ox_add;
-    const size_t opix = ((size_t)nimg * e.oH + py) * e.oW + px;
-    const size_t oplane = (size_t)e.oH * e.oW, opl_pix = (size_t)py * e.oW + px;
-    const size_t so = e.os_hi ? ((size_t)(nimg * e.os_Hp + oy + e.os_pt) * e.os_Wp + ox + e.os_pl) * e.os_pitch + e.os_coff : 0;
-    auto at = [&](const float* b, int cs, int coff, int planar, int c) -> const float* {
-      return planar ? b + ((size_t)nimg * cs + coff + c) * oplane + opl_pix : b + opix * cs + coff + c;
-    };
+    return;
+  }
+  // Fused elementwise chain.  The column-group loop is NOT unrolled: the body handles the group in r[0..3] and the registers
+  // rotate down by one group per iteration.  Unrolled over BN / 8 groups with every runtime branch, the epilogue was tens of
+  // thousands of instructions run once per tile, and fetching them, not the arithmetic or the stores, set its time.
+  int nimg[2], oy[2], ox[2];
+  bool ok[2];
 #pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    nimg[h] = oy[h] = ox[h] = 0;
+    ok[h] = rowpix(row0 + 8 * h, nimg[h], oy[h], ox[h]);
+  }
+  float r[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) r[i] = acc[i];
+  auto next_group = [&]() {
+#pragma unroll
+    for (int i = 0; i + 4 < BN / 2; ++i) r[i] = r[i + 4];
+  };
+  // two separate loops so that each keeps only its own row addresses live (registers are tight at BN = 128)
+  if (e.vec2) {
+    int opix[2], spix[2];                  // pixel indices of out / the split output in 32 bits, like e.M; element offsets in 64
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      opix[h] = (nimg[h] * e.oH + oy[h] * e.oy_mul + e.oy_add) * e.oW + ox[h] * e.ox_mul + e.ox_add;
+      spix[h] = (nimg[h] * e.os_Hp + oy[h] + e.os_pt) * e.os_Wp + ox[h] + e.os_pl;
+    }
+#pragma unroll 1
     for (int j = 0; j < BN / 8; ++j) {
       const int c = n0 + 8 * j + cl;
-      if (c >= e.Cout) continue;
-      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-      if (e.vec2) {
-        // NHWC, even channel strides / offsets, 8-byte aligned operands, Cout even: columns c, c + 1 as one float2
-        if (e.add0) { const float2 a = *reinterpret_cast<const float2*>(e.add0 + opix * e.add0_cs + e.add0_coff + c); v0 += a.x; v1 += a.y; }
-        if (e.scale) { const float2 s = __ldg(reinterpret_cast<const float2*>(e.scale + c)); v0 *= s.x; v1 *= s.y; }
-        if (e.shift) { const float2 s = __ldg(reinterpret_cast<const float2*>(e.shift + c)); v0 += s.x; v1 += s.y; }
-        v0 = act_t<ACT>(v0, e.act); v1 = act_t<ACT>(v1, e.act);
-        if (e.mul1) { const float2 s = __ldg(reinterpret_cast<const float2*>(e.mul1 + c)); v0 *= s.x; v1 *= s.y; }
-        if (e.add1) { const float2 a = *reinterpret_cast<const float2*>(e.add1 + opix * e.add1_cs + e.add1_coff + c); v0 += a.x; v1 += a.y; }
-        if (e.out) *reinterpret_cast<float2*>(e.out + opix * e.out_cs + e.out_coff + c) = make_float2(v0, v1);
-        if (e.os_hi) {                       // producer -> consumer fusion: store the consumer's bf16 hi / mid operands directly
-          if (e.os_scale) {
-            const float2 s = __ldg(reinterpret_cast<const float2*>(e.os_scale + c)), t = __ldg(reinterpret_cast<const float2*>(e.os_shift + c));
-            v0 = fmaf(v0, s.x, t.x); v1 = fmaf(v1, s.y, t.y);
-            if (e.os_relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      if (c < e.Cout) {
+        // NHWC, even channel strides / offsets, 8-byte aligned operands, Cout even: columns c, c + 1 as one float2.  The loads of
+        // the group (both rows) are issued before its first store: add0 / add1 may alias out, so the compiler cannot hoist them.
+        const float2 z2 = make_float2(0.f, 0.f);
+        const float2 sc = e.scale ? __ldg(reinterpret_cast<const float2*>(e.scale + c)) : z2;
+        const float2 sh = e.shift ? __ldg(reinterpret_cast<const float2*>(e.shift + c)) : z2;
+        const float2 m1 = e.mul1 ? __ldg(reinterpret_cast<const float2*>(e.mul1 + c)) : z2;
+        float2 a0[2], a1[2];
+        auto load_row = [&](int h) {
+          a0[h] = ok[h] && e.add0 ? *reinterpret_cast<const float2*>(e.add0 + (size_t)opix[h] * e.add0_cs + e.add0_coff + c) : z2;
+          a1[h] = ok[h] && e.add1 ? *reinterpret_cast<const float2*>(e.add1 + (size_t)opix[h] * e.add1_cs + e.add1_coff + c) : z2;
+        };
+        // both rows' residual loads ahead of the first store, except where the activation leaves no registers for them at BN = 128
+        constexpr bool kBothRows = ACT != ACT_SILU && ACT != -1;
+        if (kBothRows) { load_row(0); load_row(1); }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!kBothRows) load_row(h);
+          if (!ok[h]) continue;
+          float v0 = r[2 * h], v1 = r[2 * h + 1];
+          if (e.add0) { v0 += a0[h].x; v1 += a0[h].y; }
+          if (e.scale) { v0 *= sc.x; v1 *= sc.y; }
+          if (e.shift) { v0 += sh.x; v1 += sh.y; }
+          v0 = act_t<ACT>(v0, e.act); v1 = act_t<ACT>(v1, e.act);
+          if (e.mul1) { v0 *= m1.x; v1 *= m1.y; }
+          if (e.add1) { v0 += a1[h].x; v1 += a1[h].y; }
+          if (e.out) *reinterpret_cast<float2*>(e.out + (size_t)opix[h] * e.out_cs + e.out_coff + c) = make_float2(v0, v1);
+          if (e.os_hi) {                     // producer -> consumer fusion: store the consumer's bf16 hi / mid operands directly
+            if (e.os_scale) {
+              const float2 s = __ldg(reinterpret_cast<const float2*>(e.os_scale + c)), t = __ldg(reinterpret_cast<const float2*>(e.os_shift + c));
+              v0 = fmaf(v0, s.x, t.x); v1 = fmaf(v1, s.y, t.y);
+              if (e.os_relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            }
+            uint32_t hh, mm;
+            split2(v0, v1, hh, mm);
+            const size_t so = (size_t)spix[h] * e.os_pitch + e.os_coff + c;
+            *reinterpret_cast<uint32_t*>(e.os_hi + so) = hh;
+            *reinterpret_cast<uint32_t*>(e.os_mid + so) = mm;
           }
-          uint32_t hh, mm;
-          split2(v0, v1, hh, mm);
-          *reinterpret_cast<uint32_t*>(e.os_hi + so + c) = hh;
-          *reinterpret_cast<uint32_t*>(e.os_mid + so + c) = mm;
         }
-      } else {
+      }
+      next_group();
+    }
+    return;
+  }
+  size_t opix[2], opl_pix[2], so[2];
+  const size_t oplane = (size_t)e.oH * e.oW;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int py = oy[h] * e.oy_mul + e.oy_add, px = ox[h] * e.ox_mul + e.ox_add;
+    opix[h] = ((size_t)nimg[h] * e.oH + py) * e.oW + px;
+    opl_pix[h] = (size_t)py * e.oW + px;
+    so[h] = e.os_hi ? ((size_t)(nimg[h] * e.os_Hp + oy[h] + e.os_pt) * e.os_Wp + ox[h] + e.os_pl) * e.os_pitch + e.os_coff : 0;
+  }
+#pragma unroll 1
+  for (int j = 0; j < BN / 8; ++j) {
+    const int c = n0 + 8 * j + cl;
+    if (c < e.Cout) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!ok[h]) continue;
+        auto at = [&](const float* b, int cs, int coff, int planar, int cc) -> const float* {
+          return planar ? b + ((size_t)nimg[h] * cs + coff + cc) * oplane + opl_pix[h] : b + opix[h] * cs + coff + cc;
+        };
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
           const int cc = c + q;
           if (cc >= e.Cout) break;
-          float x = q ? v1 : v0;
+          float x = r[2 * h + q];
           if (e.add0) x += *at(e.add0, e.add0_cs, e.add0_coff, e.add0_planar, cc);
           if (e.scale) x *= __ldg(e.scale + cc);
           if (e.shift) x += __ldg(e.shift + cc);
@@ -335,10 +395,11 @@ __device__ __forceinline__ void epilogue_tile(const EpiParams& e, const float (&
             if (e.os_scale) { x = fmaf(x, __ldg(e.os_scale + cc), __ldg(e.os_shift + cc)); if (e.os_relu) x = fmaxf(x, 0.f); }
             const __nv_bfloat16 hb = __float2bfloat16_rn(x);
             const __nv_bfloat16 mb = __float2bfloat16_rn(x - __bfloat162float(hb));
-            e.os_hi[so + cc] = __bfloat16_as_ushort(hb); e.os_mid[so + cc] = __bfloat16_as_ushort(mb);
+            e.os_hi[so[h] + cc] = __bfloat16_as_ushort(hb); e.os_mid[so[h] + cc] = __bfloat16_as_ushort(mb);
           }
         }
       }
     }
+    next_group();
   }
 }

@@ -7,7 +7,7 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SETTINGS = sys.argv[1:] or ["0,40,40,600", "0,20,20,600", "0,20,10,300", "1,37,17,300", "1,45,25,500", "1,30,12,200"]
+SETTINGS = sys.argv[1:] or ["1,450,450,600", "1,300,300,600", "1,600,600,600", "1,450,450,1500", "0,40,40,600"]
 for cm in SETTINGS:
     env = dict(os.environ, MITB_CM=cm)
     out = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "layer_times.py")], env=env, capture_output=True, text=True).stdout
