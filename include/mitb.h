@@ -4,6 +4,7 @@
  * torch call made by the reference at the cited line (paths relative to manga_translator/):
  *
  *   mitb_dbnet_forward[_u8]  <- det_batch_forward_default: MODEL(batch); db.sigmoid()   detection/dbnet_convnext.py:499-509
+ *   mitb_dbnet_r34_forward[_u8] <- det_batch_forward_default of the default detector     detection/default.py:15-25
  *   mitb_ocr_forward[_u8]    <- OCR.decode up to the host loop: backbone, encoders, heads,
  *                               log_softmax + max, colour clamp                           ocr/model_48px_ctc.py:447-463
  *   mitb_lama_forward        <- LamaFourier.__call__ (inpaint_only): MPE embed, generator,
@@ -71,6 +72,17 @@ int mitb_dbnet_forward(mitb_ctx* ctx, const float* x, int n, int h, int w, float
 /* Same, input uint8 NHWC [n,h,w,3] on the device; the u8/127.5-1 normalisation is fused into the first kernel. */
 int mitb_dbnet_forward_u8(mitb_ctx* ctx, const uint8_t* img, int n, int h, int w, float* db, float* mask, void* stream);
 
+/* ---- DBNet-ResNet34 text detector, the reference's `default` detector (state_dict keys of TextDetection,
+ *      detection/default_utils/DBNet_resnet34.py:76-101; backbone.fc.* is ignored).  Its own model slot: it can be resident next
+ *      to the DBNet-ConvNeXt detector in one context. ---- */
+int mitb_dbnet_r34_load(mitb_ctx* ctx, const mitb_tensor* weights, int n_weights);
+int mitb_dbnet_r34_unload(mitb_ctx* ctx);
+/* x: [n,3,h,w] already normalised (u8/127.5-1), h and w multiples of 256 (the coarsest map is 1/256; DBNet_resnet34.py:103-125).
+ * db: [n,2,h,w] = sigmoid(DBHead output) (channel 1 is sigmoid applied twice, as default.py:23 does); mask: [n,1,h/2,w/2]. */
+int mitb_dbnet_r34_forward(mitb_ctx* ctx, const float* x, int n, int h, int w, float* db, float* mask, void* stream);
+/* Same, input uint8 NHWC [n,h,w,3] on the device; the u8/127.5-1 normalisation is fused into the first kernel. */
+int mitb_dbnet_r34_forward_u8(mitb_ctx* ctx, const uint8_t* img, int n, int h, int w, float* db, float* mask, void* stream);
+
 /* ---- 48px ResNet+Transformer CTC recogniser (state_dict keys of OCR, model_48px_ctc.py:425-436) ---- */
 int mitb_ocr_load(mitb_ctx* ctx, const mitb_tensor* weights, int n_weights);
 int mitb_ocr_unload(mitb_ctx* ctx);
@@ -121,6 +133,8 @@ int mitb_op_conv_transpose2d(mitb_ctx* ctx, const float* x, int n, int cin, int 
 /* depthwise 7x7 (pad 3, bias) + LayerNorm over C (eps), NCHW in/out. */
 int mitb_op_dwconv7_ln(mitb_ctx* ctx, const float* x, int n, int c, int h, int w, const float* wdw, const float* bdw,
                        const float* lnw, const float* lnb, float eps, float* y, void* stream);
+/* MaxPool2d(3, stride 2, padding 1) (the ResNet stem's pool), NCHW in [n,c,h,w], out [n,c,(h-1)/2+1,(w-1)/2+1]; exact. */
+int mitb_op_maxpool3x3s2(mitb_ctx* ctx, const float* x, int n, int c, int h, int w, float* y, void* stream);
 /* LayerNorm over the last dim of [rows, c]. */
 int mitb_op_layernorm(mitb_ctx* ctx, const float* x, int rows, int c, const float* w, const float* b, float eps,
                       float* y, void* stream);

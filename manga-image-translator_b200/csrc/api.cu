@@ -60,6 +60,7 @@ void mitb_destroy(mitb_ctx* ctx) {
   cudaSetDevice(ctx->c.device);
   cudaDeviceSynchronize();
   if (ctx->c.dbnet) dbnet_free(ctx->c.dbnet);
+  if (ctx->c.dbnet_r34) dbnet_r34_free(ctx->c.dbnet_r34);
   if (ctx->c.ocr) ocr_free(ctx->c.ocr);
   if (ctx->c.lama) lama_free(ctx->c.lama);
   if (ctx->c.ws.base) cudaFree(ctx->c.ws.base);
@@ -111,6 +112,34 @@ int mitb_dbnet_forward_u8(mitb_ctx* ctx, const uint8_t* img, int n, int h, int w
   MITB_CHECK(ctx->c.dbnet, "dbnet: forward before load");
   MITB_CHECK(img && db && mask, "dbnet: null buffer");
   dbnet_run(ctx->c, *ctx->c.dbnet, nullptr, img, n, h, w, db, mask, (cudaStream_t)stream);
+  API_END(ctx)
+}
+
+int mitb_dbnet_r34_load(mitb_ctx* ctx, const mitb_tensor* w, int n) {
+  API_BEGIN(ctx)
+  if (ctx->c.dbnet_r34) { dbnet_r34_free(ctx->c.dbnet_r34); ctx->c.dbnet_r34 = nullptr; }
+  Weights W = collect(w, n);
+  ctx->c.dbnet_r34 = dbnet_r34_build(ctx->c, W);
+  API_END(ctx)
+}
+int mitb_dbnet_r34_unload(mitb_ctx* ctx) {
+  API_BEGIN(ctx)
+  CUDA_OK(cudaDeviceSynchronize());
+  if (ctx->c.dbnet_r34) { dbnet_r34_free(ctx->c.dbnet_r34); ctx->c.dbnet_r34 = nullptr; }
+  API_END(ctx)
+}
+int mitb_dbnet_r34_forward(mitb_ctx* ctx, const float* x, int n, int h, int w, float* db, float* mask, void* stream) {
+  API_BEGIN(ctx)
+  MITB_CHECK(ctx->c.dbnet_r34, "dbnet_r34: forward before load");
+  MITB_CHECK(x && db && mask, "dbnet_r34: null buffer");
+  dbnet_r34_run(ctx->c, *ctx->c.dbnet_r34, x, nullptr, n, h, w, db, mask, (cudaStream_t)stream);
+  API_END(ctx)
+}
+int mitb_dbnet_r34_forward_u8(mitb_ctx* ctx, const uint8_t* img, int n, int h, int w, float* db, float* mask, void* stream) {
+  API_BEGIN(ctx)
+  MITB_CHECK(ctx->c.dbnet_r34, "dbnet_r34: forward before load");
+  MITB_CHECK(img && db && mask, "dbnet_r34: null buffer");
+  dbnet_r34_run(ctx->c, *ctx->c.dbnet_r34, nullptr, img, n, h, w, db, mask, (cudaStream_t)stream);
   API_END(ctx)
 }
 
@@ -262,6 +291,24 @@ int mitb_op_dwconv7_ln(mitb_ctx* ctx, const float* x, int n, int c, int h, int w
     if (!e.dry) launch_nchw_to_nhwc(x, n, c, h, w, xin, st);
     e.dwconv7_ln(xin, yout, wr, bdw, lnw, lnb, eps);
     if (!e.dry) launch_nhwc_to_nchw(yout, y, st);
+  });
+  CUDA_OK(cudaStreamSynchronize(st));
+  API_END(ctx)
+}
+
+int mitb_op_maxpool3x3s2(mitb_ctx* ctx, const float* x, int n, int c, int h, int w, float* y, void* stream) {
+  API_BEGIN(ctx)
+  cudaStream_t st = (cudaStream_t)stream;
+  MITB_CHECK(x && y && n >= 1 && c >= 1 && h >= 1 && w >= 1, "maxpool3x3s2: bad arguments");
+  const int ho = (h - 1) / 2 + 1, wo = (w - 1) / 2 + 1, c4 = (c + 3) & ~3;
+  run_with_workspace(ctx->c, st, [&](Exec& e) {
+    Arena& ws = e.ws();
+    View xin = ws.view(n, h, w, c4), yout = ws.view(n, ho, wo, c4);      // channels c..c4 are zero filled and dropped
+    if (!e.dry) {
+      launch_nchw_to_nhwc(x, n, c, h, w, xin, st);
+      launch_maxpool3x3s2(xin, yout, st);
+      launch_nhwc_to_nchw(yout.slice(0, c), y, st);
+    }
   });
   CUDA_OK(cudaStreamSynchronize(st));
   API_END(ctx)

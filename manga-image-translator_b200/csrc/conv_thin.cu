@@ -185,17 +185,21 @@ void launch_conv_thin(const ConvOp& op, cudaStream_t st) {
 // (py=1: rows i+1, i).
 namespace mitb {
 namespace {
-constexpr int CT_T = 16, CT_PITCH = 36;          // tile edge (input positions), padded channel pitch (floats) for Cin = 32
+constexpr int CT_T = 16;                          // tile edge (input positions)
 
+// CIN = 32 (DBNet-ConvNeXt head) or 16 (DBNet-ResNet34 head); channel pitch CIN + 4 floats
+template <int CIN>
 __global__ void __launch_bounds__(256) convT4_c1_kernel(const float* in, int H, int W, int in_cs, int in_coff, const float* w,
                                                         const float* bias, int act, float* out, int out_cs, int out_coff) {
-  __shared__ __align__(16) float tile[(CT_T + 2) * (CT_T + 2) * CT_PITCH];     // 18*18*36*4 = 46656 B
-  __shared__ __align__(16) float wsm[16 * 32];                                  // [ky*4+kx][cin]
+  static_assert(CIN == 32 || CIN == 16, "convT4_c1: Cin 32 or 16");
+  constexpr int CT_PITCH = CIN + 4, C4 = CIN / 4, LOG_CIN = CIN == 32 ? 5 : 4, LOG_C4 = LOG_CIN - 2;
+  __shared__ __align__(16) float tile[(CT_T + 2) * (CT_T + 2) * CT_PITCH];     // CIN = 32: 18*18*36*4 = 46656 B
+  __shared__ __align__(16) float wsm[16 * CIN];                                 // [ky*4+kx][cin]
   const int n = blockIdx.z, i0 = blockIdx.y * CT_T, j0 = blockIdx.x * CT_T;
   const int tid = threadIdx.x;
-  for (int t = tid; t < 16 * 32; t += 256) { const int c = t & 31, k = t >> 5; wsm[k * 32 + c] = w[c * 16 + k]; }
-  for (int t = tid; t < (CT_T + 2) * (CT_T + 2) * 8; t += 256) {
-    const int c4 = t & 7, pp = t >> 3;
+  for (int t = tid; t < 16 * CIN; t += 256) { const int c = t & (CIN - 1), k = t >> LOG_CIN; wsm[k * CIN + c] = w[c * 16 + k]; }
+  for (int t = tid; t < (CT_T + 2) * (CT_T + 2) * C4; t += 256) {
+    const int c4 = t & (C4 - 1), pp = t >> LOG_C4;
     const int ty = pp / (CT_T + 2), tx = pp - ty * (CT_T + 2);
     const int gy = i0 + ty - 1, gx = j0 + tx - 1;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -219,10 +223,10 @@ __global__ void __launch_bounds__(256) convT4_c1_kernel(const float* in, int H, 
           const int ky = py == 0 ? 1 + 2 * a : 2 * a, dy = (py + 1 - ky) / 2;      // exact: (py+1-ky) is even
           const int kx = px == 0 ? 1 + 2 * b : 2 * b, dx = (px + 1 - kx) / 2;
           const float* src = &tile[((ly + 1 + dy) * (CT_T + 2) + (lx + 1 + dx)) * CT_PITCH];
-          const float* wk = &wsm[(ky * 4 + kx) * 32];
+          const float* wk = &wsm[(ky * 4 + kx) * CIN];
           float s = 0.f;
 #pragma unroll
-          for (int c = 0; c < 32; c += 4) {
+          for (int c = 0; c < CIN; c += 4) {
             const float4 x = *reinterpret_cast<const float4*>(src + c), ww = *reinterpret_cast<const float4*>(wk + c);
             s = fmaf(x.x, ww.x, s); s = fmaf(x.y, ww.y, s); s = fmaf(x.z, ww.z, s); s = fmaf(x.w, ww.w, s);
           }
@@ -241,13 +245,14 @@ __global__ void __launch_bounds__(256) convT4_c1_kernel(const float* in, int H, 
 }
 }  // namespace
 
-// in: NHWC view with 32 channels; w: ConvTranspose2d weight [32,1,4,4] (PyTorch layout, fp32 device); out: planar view, C == 1
+// in: NHWC view with 32 or 16 channels; w: ConvTranspose2d weight [Cin,1,4,4] (PyTorch layout, fp32 device); out: planar view, C == 1
 void launch_convT4_c1(const View& in, const float* w, const float* bias, int act, const View& out, cudaStream_t st) {
-  MITB_CHECK(!in.planar && in.C == 32 && in.cs % 4 == 0 && in.coff % 4 == 0, "convT4_c1 expects a 32-channel NHWC input");
+  MITB_CHECK(!in.planar && (in.C == 32 || in.C == 16) && in.cs % 4 == 0 && in.coff % 4 == 0, "convT4_c1 expects a 32- or 16-channel NHWC input");
   MITB_CHECK(out.planar && out.C == 1 && out.H == 2 * in.H && out.W == 2 * in.W && out.N == in.N, "convT4_c1 output shape");
   dim3 grid((in.W + CT_T - 1) / CT_T, (in.H + CT_T - 1) / CT_T, in.N);
-  ProfScope ps("convT4_c1", 2.0 * in.pixels() * 4 * 4 * 32, 4.0 * (in.pixels() * 32 + in.pixels() * 4), st);
-  convT4_c1_kernel<<<grid, 256, 0, st>>>(in.p, in.H, in.W, in.cs, in.coff, w, bias, act, out.p, out.cs, out.coff);
+  ProfScope ps("convT4_c1", 2.0 * in.pixels() * 4 * 4 * in.C, 4.0 * (in.pixels() * in.C + in.pixels() * 4), st);
+  if (in.C == 32) convT4_c1_kernel<32><<<grid, 256, 0, st>>>(in.p, in.H, in.W, in.cs, in.coff, w, bias, act, out.p, out.cs, out.coff);
+  else convT4_c1_kernel<16><<<grid, 256, 0, st>>>(in.p, in.H, in.W, in.cs, in.coff, w, bias, act, out.p, out.cs, out.coff);
   count_launch();
   CUDA_OK(cudaGetLastError());
 }

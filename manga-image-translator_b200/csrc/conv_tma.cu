@@ -379,11 +379,13 @@ void make_act_tmap(CUtensorMap* m, const uint16_t* base, int N, int Hp, int Wp, 
 // Stem map over the 8-channel-padded tensor [N][Hp][Wp][8]: dimension 0 = 64 consecutive elements = an 8-pixel x 8-channel window,
 // dimension 1 = the window's first pixel with a stride of ONE pixel (16 bytes) - consecutive windows overlap by 7 pixels, which a
 // tensor map is free to describe (addresses are just sum(coord * stride)).  One box row = one output pixel's kernel row.
-bool make_stem_tmap(CUtensorMap* m, const uint16_t* base, int N, int Hp, int Wp, int bw, int bh) {
+// Stride-2 stems take every second window and row through element strides of 2 on dimensions 1 and 2 (box 2bw x 2bh, as
+// make_act_tmap does for strided convs); the smem tile is the same bw x bh windows.
+bool make_stem_tmap(CUtensorMap* m, const uint16_t* base, int N, int Hp, int Wp, int bw, int bh, int s) {
   const cuuint64_t gdim[4] = {64, (cuuint64_t)(Wp - 7), (cuuint64_t)Hp, (cuuint64_t)N};
   const cuuint64_t gstride[3] = {16, (cuuint64_t)Wp * 16, (cuuint64_t)Hp * Wp * 16};
-  const cuuint32_t box[4] = {64, (cuuint32_t)bw, (cuuint32_t)bh, 1};
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  const cuuint32_t box[4] = {64, (cuuint32_t)(bw * s), (cuuint32_t)(bh * s), 1};
+  const cuuint32_t estr[4] = {1, (cuuint32_t)s, (cuuint32_t)s, 1};
   return encode_fn()(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)base, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
@@ -513,7 +515,8 @@ bool conv_stem8_supported(const ConvOp& op) {
   static int env = -1;
   if (env < 0) { const char* e = getenv("MITB_NO_STEM8"); env = (e && atoi(e)) ? 0 : 1; }
   if (!g_tma_enabled || !env || g_stem_map_failed || !op.w8h || !op.w8m) return false;
-  if (op.in.C != 4 || op.in.planar || op.sx != 1 || op.sy != 1 || op.ntaps != op.w8_kh * op.w8_kw) return false;
+  // strides 1 and 2 only (the ConvNeXt 4x4 s4 stem keeps the gather kernel)
+  if (op.in.C != 4 || op.in.planar || op.sx != op.sy || (op.sx != 1 && op.sx != 2) || op.ntaps != op.w8_kh * op.w8_kw) return false;
   if ((op.in.cs | op.in.coff) & 3) return false;
   if (op.in_sv.valid() || op.seg2.sv.valid() || op.stat_max || op.out.C <= 4) return false;
   if (op.pad == PAD_REFLECT && (-op.tdy[0] >= op.in.H || -op.tdx[0] >= op.in.W)) return false;
@@ -624,7 +627,7 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
   }
   p.bw_log2 = 0; while ((1 << p.bw_log2) < bw) ++p.bw_log2;
   if (stem) {
-    if (!make_stem_tmap(&p.seg[0].ta_hi, sv.hi, N, sv.Hp, sv.Wp, bw, bh) || !make_stem_tmap(&p.seg[0].ta_mid, sv.mid, N, sv.Hp, sv.Wp, bw, bh)) {
+    if (!make_stem_tmap(&p.seg[0].ta_hi, sv.hi, N, sv.Hp, sv.Wp, bw, bh, op.sx) || !make_stem_tmap(&p.seg[0].ta_mid, sv.mid, N, sv.Hp, sv.Wp, bw, bh, op.sx)) {
       g_stem_map_failed = true;                                        // fall back for good: conv_stem8_supported() is false from now on
       launch_conv(op, st);
       return;

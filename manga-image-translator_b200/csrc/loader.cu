@@ -157,6 +157,32 @@ void Loader::bn_fold(const std::string& p, float eps, const float** scale, const
   *scale = ds; *shift = dh;
 }
 
+ConvW Loader::conv_bn(const std::string& wname, const std::string& p, int pad, float eps) {
+  const mitb_tensor& t = W.get(wname);
+  MITB_CHECK(t.ndim == 4, "%s: expected a Conv2d weight", wname.c_str());
+  const int Cout = (int)t.shape[0], Cin = (int)t.shape[1], kh = (int)t.shape[2], kw = (int)t.shape[3];
+  ConvW cw; cw.Cin = Cin; cw.Cout = Cout; cw.ntaps = kh * kw; cw.ldw = round4(Cout);
+  MITB_CHECK(cw.ntaps <= kMaxTaps, "%s: kernel too large", wname.c_str());
+  MITB_CHECK((int)W.get(p + "weight").shape[0] == Cout, "%s: BatchNorm has the wrong channel count", p.c_str());
+  std::vector<int> ky(cw.ntaps), kx(cw.ntaps);
+  for (int i = 0; i < cw.ntaps; ++i) { ky[i] = i / kw; kx[i] = i % kw; cw.tdy[i] = (int8_t)(ky[i] - pad); cw.tdx[i] = (int8_t)(kx[i] - pad); }
+  const size_t n = (size_t)cw.ntaps * Cin * cw.ldw;
+  float* dst = blob.alloc_f(n);
+  launch_repack(dst, t.data, Cout, Cin, cw.ntaps, ky.data(), kx.data(), (long)Cin * kh * kw, (long)kh * kw, kw, 1, cw.ldw, st);
+  const float* dscale; const float* dshift;
+  bn_fold(p, eps, &dscale, &dshift);
+  std::vector<float> sc(Cout), w(n);
+  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(cudaMemcpy(sc.data(), dscale, Cout * sizeof(float), cudaMemcpyDeviceToHost));
+  CUDA_OK(cudaMemcpy(w.data(), dst, n * sizeof(float), cudaMemcpyDeviceToHost));
+  for (size_t r = 0; r < n / cw.ldw; ++r)
+    for (int co = 0; co < Cout; ++co) w[r * cw.ldw + co] *= sc[co];
+  CUDA_OK(cudaMemcpy(dst, w.data(), n * sizeof(float), cudaMemcpyHostToDevice));
+  cw.w = dst; cw.shift = dshift;
+  conv_tc_prepare(cw, blob, st);
+  return cw;
+}
+
 float Loader::scalar(const std::string& name) {
   float v = 0.f;
   CUDA_OK(cudaMemcpy(&v, W.get(name).data, sizeof(float), cudaMemcpyDeviceToHost));

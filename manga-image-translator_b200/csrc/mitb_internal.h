@@ -143,7 +143,9 @@ void launch_layernorm(const View& in, const View& out, const float* w, const flo
 void launch_dwconv7_ln(const View& in, const View& out, const float* wdw /*[49][C]*/, const float* bdw,
                        const float* lnw, const float* lnb, float eps, cudaStream_t st, const SplitView* osv = nullptr);
 void launch_avgpool(const View& in, const View& out, int mode /*0: 2x2s2, 1: k2 s(2,1) p(0,1)*/, cudaStream_t st);
-void launch_convT4_c1(const View& in, const float* w, const float* bias, int act, const View& out, cudaStream_t st);
+// MaxPool2d(3, 2, 1); out.p may be null when osv (the consumer conv's dense bf16 hi/mid operands) is given
+void launch_maxpool3x3s2(const View& in, const View& out, cudaStream_t st, const SplitView* osv = nullptr);
+void launch_convT4_c1(const View& in, const float* w, const float* bias, int act, const View& out, cudaStream_t st);   // Cin 32 or 16
 void launch_nchw_to_nhwc(const float* src, int N, int C, int H, int W, const View& dst, cudaStream_t st);
 void launch_nhwc_to_nchw(const View& src, float* dst, cudaStream_t st);
 void launch_u8_to_nhwc(const uint8_t* src, int N, int H, int W, int C, const View& dst, float mul, float add,
@@ -242,6 +244,10 @@ struct Loader {                        // helpers used by the network builders a
   const float* vec(const std::string& name);                    // copy a 1-D tensor
   const float* vec_tiled(const std::string& name, int reps);
   void bn_fold(const std::string& prefix, float eps, const float** scale, const float** shift);
+  // Conv2d (no bias, zero padding `pad`) followed by an eval BatchNorm: the BN scale is folded into the fp32 K-major weights before
+  // the tensor-core copies are made, the BN shift becomes ConvW::shift (scale stays null).  For epilogues that add a residual
+  // BEFORE the affine (v = acc + add0; v*scale + shift): post-activation ResNet blocks, relu(bn2(conv2(.)) + identity).
+  ConvW conv_bn(const std::string& wname, const std::string& bn_prefix, int pad, float eps);
   float scalar(const std::string& name);
 };
 
@@ -252,6 +258,11 @@ DbnetModel* dbnet_build(Ctx&, const Weights&);
 void dbnet_free(DbnetModel*);
 void dbnet_run(Ctx&, DbnetModel&, const float* x_nchw, const uint8_t* x_u8, int n, int h, int w, float* db,
                float* mask, cudaStream_t st);
+struct DbnetR34Model;
+DbnetR34Model* dbnet_r34_build(Ctx&, const Weights&);
+void dbnet_r34_free(DbnetR34Model*);
+void dbnet_r34_run(Ctx&, DbnetR34Model&, const float* x_nchw, const uint8_t* x_u8, int n, int h, int w, float* db, float* mask,
+                   cudaStream_t st);
 OcrModel* ocr_build(Ctx&, const Weights&);
 void ocr_free(OcrModel*);
 void ocr_run(Ctx&, OcrModel&, const float* x_nchw, const uint8_t* x_u8, int n, int wp, int* idx, float* logprob,
@@ -284,6 +295,7 @@ struct Ctx {
   std::string err;
   Arena ws;
   DbnetModel* dbnet = nullptr; OcrModel* ocr = nullptr; LamaModel* lama = nullptr;
+  DbnetR34Model* dbnet_r34 = nullptr;  // the default detector: its own slot, so both detectors can be resident
   long launches = 0;                   // kernels launched by this library (bench.py "gpu_launches")
   void ensure_ws(size_t bytes);
 };

@@ -286,6 +286,61 @@ void launch_avgpool(const View& in, const View& out, int mode, cudaStream_t st) 
 }
 
 // ---------------------------------------------------------------------------------------------------
+// MaxPool2d(3, 2, 1) of the ResNet stem (torchvision resnet.py, -inf padding: only in-image taps compete), one thread per 4 channels
+// of an output pixel.  Max is exact, so the result equals F.max_pool2d bit for bit (a NaN wins, as in PyTorch).  Optionally it
+// also writes the result as the next conv's bf16 hi/mid operands (dense [N][Ho][Wo][C]), like launch_layernorm's osv.
+__global__ void maxpool3x3s2_kernel(const float* in, int in_cs, int in_coff, float* out, int out_cs, int out_coff, int N, int H, int W,
+                                    int C4, int Ho, int Wo, uint16_t* o_hi, uint16_t* o_mid, int o_pitch) {
+  const long total = (long)N * Ho * Wo * C4;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C4) * 4; const long pix = i / C4;
+    const int ox = (int)(pix % Wo); long r = pix / Wo; const int oy = (int)(r % Ho); const int n = (int)(r / Ho);
+    float m[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+    for (int dy = -1; dy <= 1; ++dy) {
+      const int iy = 2 * oy + dy;
+      if (iy < 0 || iy >= H) continue;
+      for (int dx = -1; dx <= 1; ++dx) {
+        const int ix = 2 * ox + dx;
+        if (ix < 0 || ix >= W) continue;
+        const float4 v = __ldg(reinterpret_cast<const float4*>(in + ((size_t)(n * H + iy) * W + ix) * in_cs + in_coff + c));
+        const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) if (e[k] > m[k] || isnan(e[k])) m[k] = e[k];
+      }
+    }
+    const float4 o = make_float4(m[0], m[1], m[2], m[3]);
+    if (out) *reinterpret_cast<float4*>(out + (size_t)pix * out_cs + out_coff + c) = o;
+    if (o_hi) {
+      uint2 hh, mm;
+      split4_bf16(o, hh, mm);
+      *reinterpret_cast<uint2*>(o_hi + (size_t)pix * o_pitch + c) = hh;
+      *reinterpret_cast<uint2*>(o_mid + (size_t)pix * o_pitch + c) = mm;
+    }
+  }
+}
+
+void launch_maxpool3x3s2(const View& in, const View& out, cudaStream_t st, const SplitView* osv) {
+  MITB_CHECK(!in.planar && !out.planar && in.C % 4 == 0 && in.cs % 4 == 0 && in.coff % 4 == 0 && out.cs % 4 == 0 && out.coff % 4 == 0,
+             "maxpool3x3s2: NHWC views with channel counts / offsets in multiples of 4");
+  const int Ho = (in.H - 1) / 2 + 1, Wo = (in.W - 1) / 2 + 1;
+  MITB_CHECK(out.N == in.N && out.H == Ho && out.W == Wo && out.C == in.C, "maxpool3x3s2: output must be [%d,%d,%d,%d]", in.N, Ho, Wo, in.C);
+  uint16_t* ohi = nullptr; uint16_t* omid = nullptr;
+  if (osv && osv->valid()) {
+    MITB_CHECK(osv->C == in.C && osv->N == in.N && osv->H == Ho && osv->W == Wo && osv->Hp == Ho && osv->Wp == Wo, "maxpool3x3s2: split output mismatch");
+    ohi = osv->hi; omid = osv->mid;
+  }
+  MITB_CHECK(out.p || ohi, "maxpool3x3s2: no output");
+  const long total = (long)in.N * Ho * Wo * (in.C / 4);
+  if (total == 0) return;
+  int blocks = (int)((total + 255) / 256); if (blocks > device_sm_count() * 32) blocks = device_sm_count() * 32;
+  // 9 comparisons per output element; reads the input (each element about 2.25 times, mostly from L2) once from HBM, writes fp32 and / or hi+mid
+  ProfScope ps("maxpool3x3s2", 9.0 * total * 4, 4.0 * in.pixels() * in.C + ((out.p ? 4.0 : 0.0) + (ohi ? 4.0 : 0.0)) * total * 4, st);
+  maxpool3x3s2_kernel<<<blocks, 256, 0, st>>>(in.p, in.cs, in.coff, out.p, out.cs, out.coff, in.N, in.H, in.W, in.C / 4, Ho, Wo, ohi, omid,
+                                              ohi ? osv->C : 0);
+  LAUNCH_END();
+}
+
+// ---------------------------------------------------------------------------------------------------
 // layout conversions.  NCHW -> NHWC view (missing channels of the view are zero-filled, e.g. RGB -> 4 channels).
 __global__ void nchw_to_nhwc_kernel(const float* src, int N, int C, int H, int W, float* dst, int cs, int coff, int Cv) {
   const long total = (long)N * H * W;

@@ -40,6 +40,10 @@ SIGNATURES = {
     "mitb_dbnet_unload": (I, [P]),
     "mitb_dbnet_forward": (I, [P, P, I, I, I, P, P, P]),
     "mitb_dbnet_forward_u8": (I, [P, P, I, I, I, P, P, P]),
+    "mitb_dbnet_r34_load": (I, [P, C.POINTER(MitbTensor), I]),
+    "mitb_dbnet_r34_unload": (I, [P]),
+    "mitb_dbnet_r34_forward": (I, [P, P, I, I, I, P, P, P]),
+    "mitb_dbnet_r34_forward_u8": (I, [P, P, I, I, I, P, P, P]),
     "mitb_ocr_load": (I, [P, C.POINTER(MitbTensor), I]),
     "mitb_ocr_unload": (I, [P]),
     "mitb_ocr_timesteps": (I, [I]),
@@ -53,6 +57,7 @@ SIGNATURES = {
     "mitb_op_conv2d": (I, [P, P, I, I, I, I, P, I, I, I, I, I, I, I, I, P, I, P, P, I, P, P]),
     "mitb_op_conv_transpose2d": (I, [P, P, I, I, I, I, P, I, I, I, I, P, I, P, P]),
     "mitb_op_dwconv7_ln": (I, [P, P, I, I, I, I, P, P, P, P, F, P, P]),
+    "mitb_op_maxpool3x3s2": (I, [P, P, I, I, I, I, P, P]),
     "mitb_op_layernorm": (I, [P, P, I, I, P, P, F, P, P]),
     "mitb_op_rfft2": (I, [P, P, I, I, I, P, P]),
     "mitb_op_irfft2": (I, [P, P, I, I, I, P, P]),

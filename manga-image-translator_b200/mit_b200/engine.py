@@ -213,6 +213,29 @@ class Engine:
         self._call(fn, _ptr(x), n, h, w, _ptr(db), _ptr(mask), self._stream())
         return db, mask
 
+    def load_dbnet_r34(self, state_dict):
+        """The default detector's network (TextDetection, DBNet_resnet34.py); its own slot next to load_dbnet's."""
+        arr, keep = self._tensors(self._float_sd(state_dict))
+        self._call(self.lib.mitb_dbnet_r34_load, arr, len(arr))
+        torch.cuda.synchronize(self.device)
+
+    def unload_dbnet_r34(self):
+        with self._lock:          # never free a model while another thread is enqueueing its forward
+            self._check(self.lib.mitb_dbnet_r34_unload(self._h))
+
+    def dbnet_r34_forward(self, x: torch.Tensor):
+        """x: float32 [n,3,h,w] normalised, or uint8 [n,h,w,3], h and w multiples of 256; returns (db sigmoid [n,2,h,w], mask [n,1,h/2,w/2])."""
+        x = x.to(self.device).contiguous()
+        if x.dtype == torch.uint8:
+            n, h, w, _ = x.shape
+        else:
+            n, _, h, w = x.shape
+        db = torch.empty((n, 2, h, w), dtype=torch.float32, device=self.device)
+        mask = torch.empty((n, 1, h // 2, w // 2), dtype=torch.float32, device=self.device)
+        fn = self.lib.mitb_dbnet_r34_forward_u8 if x.dtype == torch.uint8 else self.lib.mitb_dbnet_r34_forward
+        self._call(fn, _ptr(x), n, h, w, _ptr(db), _ptr(mask), self._stream())
+        return db, mask
+
     def load_ocr(self, state_dict, pe_table: Optional[torch.Tensor] = None):
         sd = self._float_sd(state_dict)
         sd = {k: v for k, v in sd.items() if not k.endswith("pe.pe")}
@@ -307,6 +330,14 @@ class Engine:
         y = torch.empty_like(x)
         self._call(self.lib.mitb_op_dwconv7_ln, _ptr(x), n, c, h, w, _ptr(wdw), _ptr(bdw), _ptr(lnw), _ptr(lnb),
                                                 eps, _ptr(y), self._stream())
+        return y
+
+    def maxpool3x3s2(self, x):
+        """F.max_pool2d(x, 3, 2, 1) of an NCHW float32 tensor (exact)."""
+        x = self._dev(x)
+        n, c, h, w = x.shape
+        y = torch.empty((n, c, (h - 1) // 2 + 1, (w - 1) // 2 + 1), dtype=torch.float32, device=self.device)
+        self._call(self.lib.mitb_op_maxpool3x3s2, _ptr(x), n, c, h, w, _ptr(y), self._stream())
         return y
 
     def layernorm(self, x, w, b, eps):

@@ -1,6 +1,7 @@
 """Drop-in plugin classes for the three dense-inference stages, same names / signatures / return types as the reference:
 
   DBConvNextDetector   manga_translator/detection/dbnet_convnext.py:512-588
+  DefaultDetector      manga_translator/detection/default.py:27-103 (DBNet-ResNet34; same host glue as DBConvNextDetector)
   Model48pxCTCOCR      manga_translator/ocr/model_48px_ctc.py:18-160
   LamaMPEInpainter     manga_translator/inpainting/inpainting_lama_mpe.py:26-118
   LamaLargeInpainter   manga_translator/inpainting/inpainting_lama_mpe.py:121-136
@@ -59,14 +60,24 @@ class DBConvNextDetector(_InjectableWeights, OfflineDetector):
         sd = self._injected
         if sd is None:
             sd = torch.load(self._get_file_path(self._CKPT), map_location="cpu")
-        self.engine.load_dbnet(sd["model"] if "model" in sd else sd)
+        self._load_net(sd["model"] if "model" in sd else sd)
 
     async def _unload(self):
+        self._unload_net()
+
+    # the network behind the shared `_infer` glue: one hook to load it, one to unload it, one to run a device batch
+    def _load_net(self, sd):
+        self.engine.load_dbnet(sd)
+
+    def _unload_net(self):
         self.engine.unload_dbnet()
+
+    def _net_forward(self, batch):
+        return self.engine.dbnet_forward(batch)
 
     def _batch_forward(self, batch_u8: np.ndarray):
         """det_batch_forward_default (dbnet_convnext.py:499-509) on uint8 NHWC: normalise + forward + sigmoid on device."""
-        db, mask = self.engine.dbnet_forward(self.engine.h2d(np.ascontiguousarray(batch_u8)))
+        db, mask = self._net_forward(self.engine.h2d(np.ascontiguousarray(batch_u8)))
         return self.engine.d2h(db), self.engine.d2h(mask)
 
     async def _infer(self, image: np.ndarray, detect_size: int, text_threshold: float, box_threshold: float,
@@ -89,7 +100,7 @@ class DBConvNextDetector(_InjectableWeights, OfflineDetector):
                 rh, rw = resized.shape[:2]
                 batch = eng.h2d(resized[None])
             ratio_h = ratio_w = 1 / target_ratio
-            db_t, mask_t = eng.dbnet_forward(batch)
+            db_t, mask_t = self._net_forward(batch)
             db, mask = eng.d2h(db_t[:, :1].contiguous(), scratch=True), eng.d2h(mask_t, scratch=True)   # consumed below, never returned
             img_resized_h, img_resized_w = rh, rw
         else:
@@ -112,6 +123,30 @@ class DBConvNextDetector(_InjectableWeights, OfflineDetector):
                 mask_resized = mask_resized[:, :-pad_w]
             raw_mask = np.clip(mask_resized * 255, 0, 255).astype(np.uint8)
         return textlines, raw_mask, None
+
+
+class DefaultDetector(DBConvNextDetector):
+    """The reference's `default` detector: DBNet-ResNet34 (detection/default_utils/DBNet_resnet34.py).  Its `_infer`
+    (default.py:56-103) is line for line DBConvNextDetector's, so only the network differs.  Unlike the reference constructor
+    (default.py:36-40) it neither creates the model directory nor moves a checkpoint found in the working directory."""
+    _MODEL_MAPPING = {
+        'model': {
+            'url': 'https://github.com/zyddnys/manga-image-translator/releases/download/beta-0.3/detect-20241225.ckpt',
+            'hash': '67ce1c4ed4793860f038c71189ba9630a7756f7683b1ee5afb69ca0687dc502e',
+            'file': '.',
+        }
+    }
+    _CKPT = "detect-20241225.ckpt"
+    _injected: Optional[dict] = None          # its own injected weights, not DBConvNextDetector's
+
+    def _load_net(self, sd):
+        self.engine.load_dbnet_r34(sd)
+
+    def _unload_net(self):
+        self.engine.unload_dbnet_r34()
+
+    def _net_forward(self, batch):
+        return self.engine.dbnet_r34_forward(batch)
 
 
 # ----------------------------------------------------------------------------------------------- OCR
@@ -322,10 +357,11 @@ class LamaLargeInpainter(LamaMPEInpainter):
 
 
 # ----------------------------------------------------------------------------------------------- registration
-def register(mask_refinement: bool = False):
+def register(mask_refinement: bool = False, default_detector: bool = False):
     """Replace the reference registry entries with the H100 plugins (needs the real manga_translator package).  With
     `mask_refinement=True` also rebind `manga_translator.manga_translator.dispatch_mask_refinement` (manga_translator.py:34, called at
-    :1356-1358) to the GPU stage of `mit_b200.mask_refinement` - same signature."""
+    :1356-1358) to the GPU stage of `mit_b200.mask_refinement` - same signature.  With `default_detector=True` also replace the
+    reference's `default` detector (DBNet-ResNet34) with DefaultDetector."""
     if not compat.HAVE_REFERENCE:
         raise MitbError("register() needs an importable manga_translator package; see INTEGRATION.md")
     from manga_translator import detection, inpainting, ocr  # type: ignore
@@ -338,6 +374,9 @@ def register(mask_refinement: bool = False):
     ocr.ocr_cache.pop(Ocr.ocr48px_ctc, None)
     inpainting.inpainter_cache.pop(Inpainter.lama_mpe, None)
     inpainting.inpainter_cache.pop(Inpainter.lama_large, None)
+    if default_detector:
+        detection.DETECTORS[Detector.default] = DefaultDetector
+        detection.detector_cache.pop(Detector.default, None)
     if mask_refinement:
         import manga_translator.manga_translator as mt  # type: ignore
         from . import mask_refinement as mr
