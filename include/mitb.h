@@ -206,6 +206,82 @@ int mitb_op_dilate_lines(mitb_ctx* ctx, const int32_t* lines, int nlines, int ma
 /* cv2.dilate(src, se) for a uint8 image and a ksize x ksize structuring element (anchor at the centre). */
 int mitb_op_dilate_se(mitb_ctx* ctx, const uint8_t* src, int h, int w, const uint8_t* se, int ksize, uint8_t* dst, void* stream);
 
+/* ==== test hooks (not for production use) ====
+ * One fully described convolution through the library's own dispatch, with every option of the fused conv epilogue reachable,
+ * for tests that pin that contract kernel by kernel.  The layout of both structs is fixed: the trailing "@N" comments give the
+ * byte offset of the first field declared on their line (the library checks them at compile time, a host test checks the
+ * Python mirror against them).  All pointers are device pointers.  Tensor base pointers (x, in_scale / in_shift, add0 / add1,
+ * out, every hi / mid) must be 16-byte aligned and the per-channel epilogue vectors (scale, shift, mul1, os_scale, os_shift)
+ * 4-byte aligned; unaligned channel slices are expressed through cs / coff only. */
+typedef struct {
+  const void* p;             /* NULL: unused */
+  int32_t cs, coff;          /* channel stride of the backing tensor, first channel of the slice */
+  int32_t planar;            /* backing tensor NCHW [N][cs][H][W] instead of NHWC [N][H][W][cs] */
+  int32_t reserved;
+} mitb_test_view;            /* 24 bytes */
+
+typedef struct {             /* bf16 hi / mid operand tensors [N][Hp][Wp][C], logical pixel (y, x) at (y + pt, x + pl) */
+  uint16_t* hi; uint16_t* mid;   /* hi NULL: unused */
+  int32_t C, Hp, Wp, pt, pl;     /* channel pitch, padded grid, halo offsets */
+  int32_t coff;                  /* first channel of the slice */
+} mitb_test_split;           /* 40 bytes */
+
+#define MITB_TEST_PATH_AUTO 0      /* the library's own dispatch */
+#define MITB_TEST_PATH_SIMT 1      /* tensor cores off: SIMT, fewout or thin kernel */
+#define MITB_TEST_PATH_GATHER 2    /* TMA-fed kernel off: register-gather wgmma kernel (+ split-K), or thin */
+#define MITB_TEST_PATH_TMA 3       /* must run on the TMA-fed kernel (or its Cin = 4 stem mode); an error otherwise */
+
+typedef struct {
+  /* input: fp32 NHWC (channels [coff, coff + C) of cs) or planar; x may be NULL when in_sv is given */
+  const float* x;                                                  /* @0 */
+  int32_t N, H, W, C, cs, coff, planar, in_relu;                   /* @8 */
+  const float* in_scale; const float* in_shift;                    /* @40 prologue relu?(x * in_scale + in_shift), NULL: none */
+  /* weights: PyTorch Conv2d layout [cout][wt_cin][kh][kw], wt_cin <= C (input channels beyond wt_cin get zero weights) */
+  const float* wt;                                                 /* @56 */
+  int32_t cout, wt_cin, kh, kw, stride, pad_y, pad_x, pad_mode;    /* @64 pad_mode 0 zero, 1 reflect */
+  /* epilogue v = acc (+ add0) ; v = v * scale + shift ; v = act(v) ; v *= mul1 ; v += add1 (act 0..6 as enum Act) */
+  const float* scale; const float* shift; const float* mul1;       /* @96 NULL: none */
+  int32_t act, runs;                                               /* @120 runs: launches of the same op in this call (0 = 1) */
+  mitb_test_view add0;                                             /* @128 on the output grid; add1.p == out is allowed */
+  mitb_test_view add1;                                             /* @152 */
+  /* fp32 output: grid out_H x out_W, logical output pixel (oy, ox) at (oy * oy_mul + oy_add, ox * ox_mul + ox_add) */
+  float* out;                                                      /* @176 NULL only with out_sv */
+  int32_t out_H, out_W, out_cs, out_coff, out_planar, oy_mul, oy_add, ox_mul, ox_add, reserved0;   /* @184 */
+  mitb_test_split out_sv;                                          /* @224 result also stored as bf16 hi / mid (interior) */
+  const float* os_scale; const float* os_shift;                    /* @264 applied (fmaf) before the split, NULL: none */
+  int32_t os_relu, reserved1;                                      /* @280 */
+  mitb_test_split in_sv;                                           /* @288 input given pre-split (channels [coff, coff + C)) */
+  mitb_test_split seg2;                                            /* @328 second K segment (pre-split, on the output grid) */
+  const float* seg2_wt;                                            /* @368 [cout][seg2_cin][seg2_kh][seg2_kw] */
+  int32_t seg2_cin, seg2_kh, seg2_kw, seg2_pad, seg2_pad_mode, reserved2;   /* @376 */
+  const uint8_t* need_px;                                          /* @400 uint8 [N][Ho][Wo] over the logical grid, NULL: dense */
+  int32_t path, force_bn;                                          /* @408 MITB_TEST_PATH_*; force_bn: TMA N tile (0: cost model) */
+} mitb_test_conv_desc;       /* 416 bytes */
+
+#define MITB_TEST_KERNEL_SIMT 1
+#define MITB_TEST_KERNEL_FEWOUT 2
+#define MITB_TEST_KERNEL_THIN 3
+#define MITB_TEST_KERNEL_GATHER 4
+#define MITB_TEST_KERNEL_GATHER_SPLITK 5
+#define MITB_TEST_KERNEL_TMA 6
+#define MITB_TEST_KERNEL_STEM8 7
+
+typedef struct {             /* what the last conv launch of the call ran */
+  int32_t kernel;            /* @0 MITB_TEST_KERNEL_* */
+  int32_t bn;                /* @4 N tile (fewout: Cout; thin: 0) */
+  int32_t splits;            /* @8 split-K factor (1: none) */
+  int32_t vec2;              /* @12 tensor-core epilogue: 1 float2 branch, 0 scalar branch; -1 SIMT kernels */
+  int32_t tma_act;           /* @16 conv_tma_kernel activation instantiation (enum Act, -1 runtime switch); -2 other kernels */
+  int32_t split_reused;      /* @20 launches of this call whose operand split came from the reuse cache */
+  int32_t convs;             /* @24 conv launches in this call */
+  int32_t reserved;
+} mitb_test_conv_info;       /* 32 bytes */
+
+/* Runs the conv `runs` times on `stream`, synchronises, fills *info.  Error (non-zero) for a bad descriptor, a misaligned
+ * pointer, a path that cannot take the op, or a force_bn the TMA kernel's N tile choice would never make for this cout. */
+int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* desc, mitb_test_conv_info* info, void* stream);
+int mitb_test_struct_sizes(int* desc_bytes, int* info_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,6 +19,8 @@ namespace mitb {
 
 thread_local long* g_launch_counter = nullptr;
 unsigned long g_launch_epoch = 0;
+ConvTrace* g_conv_trace = nullptr;
+int g_conv_force_bn = 0;
 
 struct ConvKParams {
   const float* in; int N, H, W, in_cs, in_coff, Cin, in_planar;
@@ -469,6 +471,7 @@ void launch_conv(const ConvOp& op, cudaStream_t st) {
     // with an output-sparsity hint the executed work depends on the mask (device data): no flop figure is claimed for that class
     const bool sparse = op.tile_mask || op.tile_mask_u8;
     ProfScope ps(sparse ? "conv7_thin_sparse" : "conv7_thin", sparse ? 0.0 : flops, sparse ? 0.0 : bytes, st, p.M, p.K, Cout);
+    conv_trace(CK_THIN, 0, 1, -1, -2, false);
     launch_conv_thin(op, st);
     return;
   }
@@ -484,9 +487,11 @@ void launch_conv(const ConvOp& op, cudaStream_t st) {
     MITB_CHECK(!op.in.planar, "row-stat epilogue expects NHWC input");
     dim3 grid((p.M + BM - 1) / BM, (Cout + 127) / 128);
     MITB_CHECK(op.stat_ld == (int)grid.y, "stat_ld must equal conv_stat_blocks(Cout)");
+    conv_trace(CK_SIMT, 128, 1, -1, -2, false);
     conv_igemm_kernel<128, false, true><<<grid, NT, 0, st>>>(p);
   } else if (Cout <= 4 && !op.in.planar && op.ldw == 4) {
     dim3 grid((p.M + 127) / 128);
+    conv_trace(CK_FEWOUT, Cout, 1, -1, -2, false);
     switch (Cout) {
       case 1: conv_fewout_kernel<1><<<grid, 128, 0, st>>>(p); break;
       case 2: conv_fewout_kernel<2><<<grid, 128, 0, st>>>(p); break;
@@ -496,6 +501,7 @@ void launch_conv(const ConvOp& op, cudaStream_t st) {
   } else {
     const int t128 = (Cout + 127) / 128 * 128, t64 = (Cout + 63) / 64 * 64;
     const bool use64 = t64 * 10 < t128 * 9;
+    conv_trace(CK_SIMT, use64 ? 64 : 128, 1, -1, -2, false);
     if (use64) {
       dim3 grid((p.M + BM - 1) / BM, (Cout + 63) / 64);
       if (op.in.planar) conv_igemm_kernel<64, true, false><<<grid, NT, 0, st>>>(p);

@@ -300,6 +300,7 @@ int pick_bn(int Cout) {
 
 static bool g_tc_enabled = true;
 void conv_tc_set_enabled(bool on) { g_tc_enabled = on; }
+bool conv_tc_enabled() { return g_tc_enabled; }
 
 // TMA descriptor of a K-major bf16 weight matrix [npad][kpad]: box = 64 k (128 bytes, SWIZZLE_128B) x BN rows.
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -469,6 +470,7 @@ void launch_conv_tc(const ConvOp& op, cudaStream_t st) {
   }
   const int total_tiles = tiles * splits;
   const int grid = total_tiles < num_sms ? total_tiles : num_sms;      // persistent: one CTA per SM
+  conv_trace(splits > 1 ? CK_GATHER_SPLITK : CK_GATHER, BN, splits, p.e.vec2, -2, false);
   switch (BN) {
     case 32: conv_tc_kernel<32><<<grid, TC_THREADS, smem, st>>>(p); break;
     case 64: conv_tc_kernel<64><<<grid, TC_THREADS, smem, st>>>(p); break;

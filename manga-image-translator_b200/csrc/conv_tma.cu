@@ -462,6 +462,12 @@ void conv_halo(const int8_t* tdy, const int8_t* tdx, int ntaps, int pad, int H, 
 }  // namespace
 
 void conv_tma_set_enabled(bool on) { g_tma_enabled = on; }
+bool conv_tma_enabled() { return g_tma_enabled; }
+bool conv_tma_bn_candidate(int Cout, int bn) {
+  for (int j = 1; j <= 16; ++j)
+    if ((((Cout + j - 1) / j + 31) & ~31) == bn && bn <= 128) return true;
+  return false;
+}
 
 void launch_split(const View& in, const SplitView& sv, int coff, const float* in_scale, const float* in_shift, int in_relu, cudaStream_t st) {
   MITB_CHECK(sv.valid() && sv.N == in.N && sv.H == in.H && sv.W == in.W && coff + in.C <= sv.C, "split: shape mismatch");
@@ -545,7 +551,7 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
     }
   };
   static SplitKey g_key; static bool g_key_valid = false; static unsigned long g_key_epoch = 0; static const uint16_t* g_key_hi = nullptr;
-  bool remember = false;
+  bool remember = false, reused = false;
   if (op.in_sv.valid()) {
     // ---- the producer already wrote this conv's bf16 hi / mid operands (ConvOp::out_sv of an earlier op, or launch_split)
     sv = op.in_sv; sv_coff = op.in_sv_coff;
@@ -580,6 +586,7 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
     const SplitKey key{op.in.p, N, H, W, C, op.in.cs, op.in.coff, op.in.planar, sv.Hp, sv.Wp, pt, pl, op.in_relu, op.in_scale, op.in_shift, st, dev};
     const bool reuse = g_key_valid && g_key_epoch == g_launch_epoch && g_key_hi == sv.hi && key.same(g_key);
     if (!reuse) launch_split(op.in, sv, 0, op.in_scale, op.in_shift, op.in_relu, st);
+    reused = reuse;
     // remember this split unless the conv writes into the tensor it was made from
     const float* ib = op.in.p; const float* ie = ib + (size_t)op.in.N * op.in.H * op.in.W * op.in.cs;
     const float* ob = op.out.p; const float* oe = ob ? ob + (size_t)op.out.N * op.out.H * op.out.W * op.out.cs : ob;
@@ -656,7 +663,11 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
   p.nkb = kdim / TC_BK;
   // ---- N tile: fixed by the row-stat layout for the vocabulary head, otherwise chosen per launch against wave quantisation
   const long mtiles = (long)p.N * p.tiles_y * p.tiles_x;
-  const int BN = op.stat_max ? op.tc_bn : choose_bn(op.out.C, mtiles, p.nkb, num_sms, op.act == ACT_GELU);
+  int BN = op.stat_max ? op.tc_bn : choose_bn(op.out.C, mtiles, p.nkb, num_sms, op.act == ACT_GELU);
+  if (g_conv_force_bn && !op.stat_max) {
+    MITB_CHECK(conv_tma_bn_candidate(op.out.C, g_conv_force_bn), "tma conv: BN %d is not a candidate N tile for Cout %d", g_conv_force_bn, op.out.C);
+    BN = g_conv_force_bn;
+  }
   MITB_CHECK(BN >= 32 && BN <= 128 && BN % 32 == 0, "tma conv: bad BN %d", BN);
   p.npad = (op.out.C + BN - 1) / BN * BN;
   make_w_tmap(&p.tb_hi, stem ? op.w8h : padded_w ? op.whp : op.wh, kdim, op.tc_npad, BN);
@@ -688,6 +699,8 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
   const size_t smem = stages * stage_bytes + 2 * stages * 8 + 1024;
   const long total_tiles = mtiles * (p.npad / BN);
   const int grid = (int)(total_tiles < num_sms ? total_tiles : num_sms);      // persistent: one CTA per SM
+  const int act_inst = op.stat_max ? ACT_NONE : (op.act == ACT_NONE || op.act == ACT_RELU || op.act == ACT_GELU || op.act == ACT_SILU) ? op.act : -1;
+  conv_trace(stem ? CK_STEM8 : CK_TMA, BN, 1, p.e.vec2, act_inst, reused);
 #define MITB_TMA_LAUNCH(A)                                                              \
   switch (BN) {                                                                        \
     case 32: conv_tma_kernel<A, 32><<<grid, TM_THREADS, smem, st>>>(p); break;          \

@@ -76,6 +76,9 @@ constexpr int kMaxTaps = 49;
 
 struct alignas(64) TmaDesc { uint64_t q[16]; };   // opaque CUtensorMap (128 bytes)
 
+// Alignment: the base pointers of in / out / add0 / add1 (and of every split tensor) must be 16-byte aligned, in_scale / in_shift
+// too: the SIMT kernel reads and writes float4 whenever cs and coff are multiples of 4 and the split kernels move 16-byte packs.
+// scale / shift / mul1 / os_scale / os_shift need 4 bytes (the tensor-core epilogue reads them as float2 only when 8-byte aligned).
 struct ConvOp {
   View in, out;                       // out grid may be larger than the logical (Ho,Wo) grid (transposed phases)
   const float* w = nullptr;           // [ntaps*Cin][ldw] K-major rows, ldw = round4(Cout)
@@ -122,6 +125,20 @@ struct ConvOp {
 };
 
 void launch_conv(const ConvOp& op, cudaStream_t st);
+// Host-side record of what launch_conv() ran (test hook mitb_test_conv): null by default, and nothing is recorded then.
+enum ConvKernel { CK_SIMT = 1, CK_FEWOUT, CK_THIN, CK_GATHER, CK_GATHER_SPLITK, CK_TMA, CK_STEM8 };
+struct ConvTrace { int kernel = 0, bn = 0, splits = 1, vec2 = -1, tma_act = -2, split_reused = 0, convs = 0; };
+extern ConvTrace* g_conv_trace;
+inline void conv_trace(int kernel, int bn, int splits, int vec2, int tma_act, bool reused) {
+  if (!g_conv_trace) return;
+  ConvTrace& t = *g_conv_trace;
+  t.kernel = kernel; t.bn = bn; t.splits = splits; t.vec2 = vec2; t.tma_act = tma_act; t.split_reused += reused ? 1 : 0; ++t.convs;
+}
+extern int g_conv_force_bn;                // non-zero: the TMA kernel's N tile (must be one of choose_bn's candidates); test hook only
+bool conv_tma_bn_candidate(int Cout, int bn);
+bool conv_tc_enabled();
+bool conv_tma_enabled();
+void conv_tma_set_enabled(bool on);
 bool conv_uses_tma(const ConvOp& op);      // true when launch_conv() will run this op on the TMA-fed tensor-core kernel
 bool conv_tma_capable(const ConvOp& op);   // the op CAN run there (launch_conv() does so whenever in_sv / out_sv / seg2 is set)
 // fill the reflect halo of channels [coff, coff+C) of a split tensor from its interior (pad <= 3)

@@ -16,6 +16,37 @@ class MitbTensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("ndim", C.c_int32), ("shape", C.c_int64 * 4)]
 
 
+class MitbTestView(C.Structure):
+    _fields_ = [("p", C.c_void_p), ("cs", C.c_int32), ("coff", C.c_int32), ("planar", C.c_int32), ("reserved", C.c_int32)]
+
+
+class MitbTestSplit(C.Structure):
+    _fields_ = [("hi", C.c_void_p), ("mid", C.c_void_p), ("C", C.c_int32), ("Hp", C.c_int32), ("Wp", C.c_int32),
+                ("pt", C.c_int32), ("pl", C.c_int32), ("coff", C.c_int32)]
+
+
+def _ints(*names):
+    return [(n, C.c_int32) for n in names]
+
+
+class MitbTestConvDesc(C.Structure):
+    """mitb_test_conv_desc (test hook, include/mitb.h): one fully described conv with every fused-epilogue option."""
+    _fields_ = ([("x", C.c_void_p)] + _ints("N", "H", "W", "C", "cs", "coff", "planar", "in_relu") +
+                [("in_scale", C.c_void_p), ("in_shift", C.c_void_p), ("wt", C.c_void_p)] +
+                _ints("cout", "wt_cin", "kh", "kw", "stride", "pad_y", "pad_x", "pad_mode") +
+                [("scale", C.c_void_p), ("shift", C.c_void_p), ("mul1", C.c_void_p)] + _ints("act", "runs") +
+                [("add0", MitbTestView), ("add1", MitbTestView), ("out", C.c_void_p)] +
+                _ints("out_H", "out_W", "out_cs", "out_coff", "out_planar", "oy_mul", "oy_add", "ox_mul", "ox_add", "reserved0") +
+                [("out_sv", MitbTestSplit), ("os_scale", C.c_void_p), ("os_shift", C.c_void_p)] + _ints("os_relu", "reserved1") +
+                [("in_sv", MitbTestSplit), ("seg2", MitbTestSplit), ("seg2_wt", C.c_void_p)] +
+                _ints("seg2_cin", "seg2_kh", "seg2_kw", "seg2_pad", "seg2_pad_mode", "reserved2") +
+                [("need_px", C.c_void_p)] + _ints("path", "force_bn"))
+
+
+class MitbTestConvInfo(C.Structure):
+    _fields_ = _ints("kernel", "bn", "splits", "vec2", "tma_act", "split_reused", "convs", "reserved")
+
+
 class MitbError(RuntimeError):
     pass
 
@@ -77,6 +108,8 @@ SIGNATURES = {
     "mitb_op_dense_crf": (I, [P, P, P, I, P, P, I, I, I, I, LL, LL, LL, I, F, F, F, F, F, F, P, P, P, P]),
     "mitb_op_dilate_lines": (I, [P, P, I, I, P, P, P, I, P, P]),
     "mitb_op_dilate_se": (I, [P, P, I, I, P, I, P, P]),
+    "mitb_test_conv": (I, [P, C.POINTER(MitbTestConvDesc), C.POINTER(MitbTestConvInfo), P]),
+    "mitb_test_struct_sizes": (I, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
 }
 
 

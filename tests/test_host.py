@@ -31,6 +31,34 @@ def test_abi_header_and_library_agree():
     assert b"sm_90a" in lib.mitb_version()
 
 
+def test_test_hook_structs_match_header():
+    """The ctypes mirrors of the conv test hook's structs have the library's sizes and the field offsets include/mitb.h states
+    ("@N" on a field's line is the offset of the first field declared there; "N bytes" after a struct is its size)."""
+    from mit_b200 import _lib
+    lib = _lib.load()
+    d, i = ctypes.c_int(), ctypes.c_int()
+    assert lib.mitb_test_struct_sizes(ctypes.byref(d), ctypes.byref(i)) == 0
+    assert (d.value, i.value) == (ctypes.sizeof(_lib.MitbTestConvDesc), ctypes.sizeof(_lib.MitbTestConvInfo))
+    hdr = open(os.path.join(ROOT, "include", "mitb.h")).read()
+    mirrors = {"mitb_test_view": _lib.MitbTestView, "mitb_test_split": _lib.MitbTestSplit,
+               "mitb_test_conv_desc": _lib.MitbTestConvDesc, "mitb_test_conv_info": _lib.MitbTestConvInfo}
+    stated = 0
+    for name, mirror in mirrors.items():
+        body, size = re.search(r"typedef struct \{([^{}]*)\}\s*" + name + r";\s*/\*\s*(\d+) bytes", hdr, re.S).groups()
+        assert ctypes.sizeof(mirror) == int(size), name
+        declared = []
+        for line in body.splitlines():
+            code = re.sub(r"/\*.*?(\*/|$)", "", line).strip()
+            fields = [re.sub(r"\[.*\]", "", f).split()[-1].lstrip("*") for f in re.split(r"[;,]", code) if f.strip()]
+            declared += fields
+            m = re.search(r"/\*\s*@(\d+)", line)
+            if m:
+                assert getattr(mirror, fields[0]).offset == int(m.group(1)), (name, fields[0])
+                stated += 1
+        assert declared == [f[0] for f in mirror._fields_], name      # same fields in the same order
+    assert stated >= 25
+
+
 def test_no_cpu_fallback():
     """Without a CUDA device context creation fails loudly (and the plugins refuse non-CUDA devices)."""
     import torch
