@@ -274,7 +274,7 @@ typedef struct {             /* what the last conv launch of the call ran */
   int32_t tma_act;           /* @16 conv_tma_kernel activation instantiation (enum Act, -1 runtime switch); -2 other kernels */
   int32_t split_reused;      /* @20 launches of this call whose operand split came from the reuse cache */
   int32_t convs;             /* @24 conv launches in this call */
-  int32_t reserved;
+  int32_t staged;            /* @28 conv_tma_kernel: channels per thread of the staged epilogue (4 or 2), 0 register epilogue; -1 other kernels */
 } mitb_test_conv_info;       /* 32 bytes */
 
 /* Runs the conv `runs` times on `stream`, synchronises, fills *info.  Error (non-zero) for a bad descriptor, a misaligned

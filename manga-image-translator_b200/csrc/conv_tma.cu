@@ -11,8 +11,9 @@
 //   warps 0-7   two consumer warpgroups in ping-pong: each owns whole 128-row tiles, alternately, and issues 24 wgmma per K
 //               block (two 64-row halves, bf16x3: Ah*Bh + Ah*Bm + Am*Bh, fp32 accumulators in registers); the stage is released
 //               on its "empty" mbarrier once the wgmma that read it retired (one K block of wgmma stays in flight); then the
-//               epilogue straight from the accumulator registers ((+add0)*scale+shift -> act -> *mul1 -> +add1 -> fp32 stores
-//               and / or split operands, tc_common.cuh) while the other warpgroup's main loop runs on the tensor core.
+//               epilogue ((+add0)*scale+shift -> act -> *mul1 -> +add1 -> fp32 stores and / or split operands), staged through
+//               shared memory (epilogue_staged) or, for planar / unaligned outputs and the vocabulary head, straight from the
+//               accumulator registers (tc_common.cuh), while the other warpgroup's main loop runs on the tensor core.
 // Operand fusion (ConvOp::in_sv / out_sv / seg2): a producer's epilogue can store its result directly as the consumer's bf16
 // hi/mid operand tensor (SplitView, optionally with a reflect halo and the consumer's BN+ReLU prologue applied), so the split
 // pass disappears; and a second K segment with its own tensor maps lets two convolutions of different inputs accumulate into one
@@ -50,6 +51,9 @@ struct TmaParams {
   int sy, sx;                                                 // conv stride (TMA element strides of the activation box)
   int bw_log2, tiles_x, tiles_y;
   int npad, stages;
+  int staged;                                                 // fused chain through epilogue_staged (stage_epilogue), else epilogue_tile
+  int bar_off;                                                // shared-memory offset of the barriers: after the stages and, if
+                                                              // the epilogue is staged, its chunks and row tables
   const uint8_t* tile_need;                                   // per 128-row M tile: 0 = skip (ConvOp::need_px reduced over the tile), null: all
   EpiParams e;
 };
@@ -68,6 +72,132 @@ template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile
 template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 __device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// ---- Staged epilogue of the fused chain (EpiParams::vec2 outputs).  In the accumulator layout a thread holds 2 columns of each
+// 8-column group in 4 rows, so a chain applied straight from the registers moves 8 bytes per row and address, and each thread has
+// few independent values to hide the latency of its loads with.  Instead each consumer warpgroup passes its tile through shared memory
+// 32 columns at a time: the fragments are written to a 128 x 32 fp32 chunk and read back row-major, each thread owning W (4, or 2
+// where the operands' alignment allows only 8 bytes) fixed channels and walking the rows.  A warp then moves whole 128-byte row
+// segments of out / add0 / add1 (64 bytes of os_hi / os_mid) per instruction, the column vectors are loaded once per chunk, and the
+// latency is hidden by rows in flight.  The element chain is epi_chain2 / epi_split2, as in epilogue_tile.
+constexpr int EPI_CW = 32;                                                   // columns per chunk
+constexpr uint32_t EPI_CHUNK_BYTES = TC_BM * EPI_CW * 4;                     // 16 KB per consumer warpgroup
+constexpr uint32_t EPI_SMEM_BYTES = 2 * (EPI_CHUNK_BYTES + TC_BM * 4);       // + per warpgroup a 128-entry row table
+
+// float offset of (row r, column col) in a chunk: the 16-byte units of a row are XOR-swizzled by r & 3, so that the fragment stores
+// (a half warp writes 32 bytes of each of 4 consecutive rows) and the row reads (8 or 16 lanes read 128 bytes of one row) are both
+// free of bank conflicts
+__device__ __forceinline__ int chunk_off(int r, int col) { return r * EPI_CW + (((col >> 2) ^ ((r & 3) << 1)) << 2) + (col & 3); }
+
+template <int W> __device__ __forceinline__ void ld_w(float (&v)[W], const float* q);
+template <> __device__ __forceinline__ void ld_w<4>(float (&v)[4], const float* q) {
+  const float4 t = *reinterpret_cast<const float4*>(q); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+}
+template <> __device__ __forceinline__ void ld_w<2>(float (&v)[2], const float* q) {
+  const float2 t = *reinterpret_cast<const float2*>(q); v[0] = t.x; v[1] = t.y;
+}
+template <int W> __device__ __forceinline__ void ldg_w(float (&v)[W], const float* q);
+template <> __device__ __forceinline__ void ldg_w<4>(float (&v)[4], const float* q) {
+  const float4 t = __ldg(reinterpret_cast<const float4*>(q)); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+}
+template <> __device__ __forceinline__ void ldg_w<2>(float (&v)[2], const float* q) {
+  const float2 t = __ldg(reinterpret_cast<const float2*>(q)); v[0] = t.x; v[1] = t.y;
+}
+template <int W> __device__ __forceinline__ void st_w(float* q, const float (&v)[W]);
+template <> __device__ __forceinline__ void st_w<4>(float* q, const float (&v)[4]) { *reinterpret_cast<float4*>(q) = make_float4(v[0], v[1], v[2], v[3]); }
+template <> __device__ __forceinline__ void st_w<2>(float* q, const float (&v)[2]) { *reinterpret_cast<float2*>(q) = make_float2(v[0], v[1]); }
+template <int W> __device__ __forceinline__ void st_bf16_w(uint16_t* q, const uint32_t (&v)[W / 2]);
+template <> __device__ __forceinline__ void st_bf16_w<4>(uint16_t* q, const uint32_t (&v)[2]) { *reinterpret_cast<uint2*>(q) = make_uint2(v[0], v[1]); }
+template <> __device__ __forceinline__ void st_bf16_w<2>(uint16_t* q, const uint32_t (&v)[1]) { *reinterpret_cast<uint32_t*>(q) = v[0]; }
+
+// The fused chain of one 128 x BN tile: acc0 holds rows 0-63, acc1 rows 64-127 (fragment layout of epilogue_tile; `row` is this
+// thread's first row); both are consumed.  rowpix(r, ...) as in epilogue_tile; rowm(r) is the tile row's index in the logical output
+// grid, which is the pixel index of out / add0 / add1 whenever there is a split output (tma_launch admits out_sv only on the conv's
+// own grid), so the row table needs one entry per row.  `bar` is this warpgroup's named barrier.
+template <int ACT, int BN, int W, class RowPix, class RowM>
+__device__ __forceinline__ void epilogue_staged(const EpiParams& e, float (&acc0)[BN / 2], float (&acc1)[BN / 2], int row, int n0, float* chunk,
+                                                int* rtab, int bar, RowPix rowpix, RowM rowm) {
+  constexpr int TPR = EPI_CW / W, RPP = TC_BM / TPR, NR = (BN == 128 ? 4 : 8) / W;   // threads per row, rows per pass, rows in flight
+  // (at BN = 128 the 96 accumulator registers still live during the first chunk leave room for one 16-byte row only: 2 spill)
+  const int t = threadIdx.x & 127, cl = 2 * (t & 3);
+  const int q = t % TPR, r0 = t / TPR;
+  named_bar_sync(bar, 128);                           // the previous tile's reads of the chunk and the row table are done
+  {
+    // row table: pixel index of the split output if there is one, else of out; -1 outside the output
+    int nimg = 0, oy = 0, ox = 0;
+    const bool ok = rowpix(t, nimg, oy, ox);
+    rtab[t] = !ok ? -1 : e.os_hi ? (nimg * e.os_Hp + oy + e.os_pt) * e.os_Wp + ox + e.os_pl
+                                 : (nimg * e.oH + oy * e.oy_mul + e.oy_add) * e.oW + ox * e.ox_mul + e.ox_add;
+  }
+#pragma unroll 1
+  for (int c0 = n0; c0 < n0 + BN && c0 < e.Cout; c0 += EPI_CW) {
+    if (c0 != n0) named_bar_sync(bar, 128);           // the previous chunk's reads are done
+    // this chunk's fragments, acc[0..15] (the registers rotate down by one chunk per iteration): columns 8 jj + cl, rows row + 8 h.
+    // The 16 store addresses are recomputed per chunk (rr is opaque to the compiler): hoisted out of the loop they would hold 16
+    // registers through it and make the BN = 128 instantiations spill.
+    int rr = row;
+    asm volatile("" : "+r"(rr));
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        *reinterpret_cast<float2*>(chunk + chunk_off(rr + 8 * h, 8 * jj + cl)) = make_float2(acc0[4 * jj + 2 * h], acc0[4 * jj + 2 * h + 1]);
+        *reinterpret_cast<float2*>(chunk + chunk_off(64 + rr + 8 * h, 8 * jj + cl)) = make_float2(acc1[4 * jj + 2 * h], acc1[4 * jj + 2 * h + 1]);
+      }
+    }
+    named_bar_sync(bar, 128);
+    const int c = c0 + W * q;                           // Cout is a multiple of W: a thread's channels are all inside or all past it
+    if (c < e.Cout) {
+      float sc[W], sh[W], m1[W], os[W], ot[W];
+#pragma unroll
+      for (int k = 0; k < W; ++k) sc[k] = sh[k] = m1[k] = os[k] = ot[k] = 0.f;
+      if (e.scale) ldg_w<W>(sc, e.scale + c);
+      if (e.shift) ldg_w<W>(sh, e.shift + c);
+      if (e.mul1) ldg_w<W>(m1, e.mul1 + c);
+      if (e.os_scale) { ldg_w<W>(os, e.os_scale + c); ldg_w<W>(ot, e.os_shift + c); }
+#pragma unroll 1
+      for (int i0 = 0; i0 < TC_BM / RPP; i0 += NR) {
+        // the residual loads of all rows in flight ahead of the first store: add0 / add1 may alias out
+        int px[NR], opx[NR];
+        float a0[NR][W], a1[NR][W];
+#pragma unroll
+        for (int i = 0; i < NR; ++i) {
+          const int r = r0 + (i0 + i) * RPP;
+          px[i] = rtab[r];
+          opx[i] = e.os_hi ? rowm(r) : px[i];
+#pragma unroll
+          for (int k = 0; k < W; ++k) a0[i][k] = a1[i][k] = 0.f;
+          if (px[i] >= 0) {
+            if (e.add0) ld_w<W>(a0[i], e.add0 + (size_t)opx[i] * e.add0_cs + e.add0_coff + c);
+            if (e.add1) ld_w<W>(a1[i], e.add1 + (size_t)opx[i] * e.add1_cs + e.add1_coff + c);
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < NR; ++i) {
+          if (px[i] < 0) continue;
+          float v[W];
+          ld_w<W>(v, chunk + chunk_off(r0 + (i0 + i) * RPP, W * q));
+#pragma unroll
+          for (int k = 0; k < W; k += 2)
+            epi_chain2<ACT>(e, v[k], v[k + 1], make_float2(a0[i][k], a0[i][k + 1]), make_float2(sc[k], sc[k + 1]), make_float2(sh[k], sh[k + 1]),
+                            make_float2(m1[k], m1[k + 1]), make_float2(a1[i][k], a1[i][k + 1]));
+          if (e.out) st_w<W>(e.out + (size_t)opx[i] * e.out_cs + e.out_coff + c, v);
+          if (e.os_hi) {
+            uint32_t hh[W / 2], mm[W / 2];
+#pragma unroll
+            for (int k = 0; k < W; k += 2)
+              epi_split2(e, v[k], v[k + 1], make_float2(os[k], os[k + 1]), make_float2(ot[k], ot[k + 1]), hh[k / 2], mm[k / 2]);
+            const size_t so = (size_t)px[i] * e.os_pitch + e.os_coff + c;
+            st_bf16_w<W>(e.os_hi + so, hh);
+            st_bf16_w<W>(e.os_mid + so, mm);
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int i = 0; i + 16 < BN / 2; ++i) { acc0[i] = acc0[i + 16]; acc1[i] = acc1[i + 16]; }
+  }
+}
 
 // expect_tx + the four operand boxes of one K block, issued by one elected lane of a converged warp
 __device__ __forceinline__ void tma_kblock(uint32_t bar, uint32_t bytes, uint32_t a_hi, uint32_t a_mid, uint32_t b_hi, uint32_t b_mid,
@@ -93,7 +223,8 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
   const int S = p.stages;
   constexpr uint32_t a_bytes = TC_BM * 128, b_bytes = (uint32_t)BN * 128;
   constexpr uint32_t stage_bytes = 2 * a_bytes + 2 * b_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);   // full[S], empty[S]
+  uint8_t* epi_smem = smem + (size_t)S * stage_bytes;                             // staged epilogue: chunks, row tables
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.bar_off);                  // full[S], empty[S]
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar_base = smem_u32(bars);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
@@ -192,8 +323,18 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
         nimg = nimg_t; oy = oy0 + (r >> p.bw_log2); ox = ox0 + (r & (bw - 1));
         return oy < p.Ho && ox < p.Wo && nimg < p.N;
       };
-      epilogue_tile<ACT, BN>(p.e, acc0, row, n0, 0, rowpix);
-      epilogue_tile<ACT, BN>(p.e, acc1, 64 + row, n0, 0, rowpix);
+      if (p.staged) {
+        auto rowm = [&](int r) -> int {
+          return p.lin ? ox0 + r : (nimg_t * p.Ho + oy0 + (r >> p.bw_log2)) * p.Wo + ox0 + (r & (bw - 1));
+        };
+        float* chunk = reinterpret_cast<float*>(epi_smem + wg * EPI_CHUNK_BYTES);
+        int* rtab = reinterpret_cast<int*>(epi_smem + 2 * EPI_CHUNK_BYTES) + wg * TC_BM;
+        if (p.e.vec4) epilogue_staged<ACT, BN, 4>(p.e, acc0, acc1, row, n0, chunk, rtab, 3 + wg, rowpix, rowm);
+        else epilogue_staged<ACT, BN, 2>(p.e, acc0, acc1, row, n0, chunk, rtab, 3 + wg, rowpix, rowm);
+      } else {
+        epilogue_tile<ACT, BN>(p.e, acc0, row, n0, 0, rowpix);
+        epilogue_tile<ACT, BN>(p.e, acc1, 64 + row, n0, 0, rowpix);
+      }
 #ifdef MITB_CONV_PHASES
       c4 = clock64();
       sum[0] += c1 - c0; sum[1] += c2 - c1; sum[2] += c3 - c2; sum[3] += c4 - c3; ++ntl;
@@ -408,23 +549,34 @@ void make_w_tmap(CUtensorMap* m, const uint16_t* base, int kdim, int rows, int b
 // 12 bn cycles (measured with tools/conv_phases.py: 1490-1660 clk per K block at bn = 128 on L2-resident layers).  The two
 // consumer warpgroups alternate whole tiles and one warpgroup's epilogue overlaps the other's main loop, so a CTA finishes two
 // tiles per max(2 main, main + epilogue): tile time = max(main, (main + epilogue) / 2) + a fixed cost (mode 1; mode 0 is the
-// sum, for a schedule without overlap).  The epilogue cycles per column are measured (tools/conv_phases.py), the L2 share (42 B/clk)
-// is an estimate; MITB_CM="mode,epi_gelu,epi,fix" overrides the constants (tools/cost_model_sweep.py).
-struct CostModel { int mode; double epi_gelu, epi, fix; };
+// sum, for a schedule without overlap).  The epilogue cycles per column are measured (tools/conv_phases.py): epi_reg for the
+// register epilogue, epi / epi_gelu for the staged one; the L2 share (42 B/clk) is an estimate.  MITB_CM="mode,epi_gelu,epi,fix,
+// epi_reg" overrides the constants (tools/cost_model_sweep.py).
+struct CostModel { int mode; double epi_gelu, epi, fix, epi_reg; };
 const CostModel& cost_model() {
-  static CostModel cm = {1, 450.0, 450.0, 600.0};
+  static CostModel cm = {1, 225.0, 350.0, 600.0, 450.0};
   static bool init = false;
   if (!init) {
     init = true;
     if (const char* e = getenv("MITB_CM")) {
-      int mode = 0; double a = 0, b = 0, c = 0;
-      if (sscanf(e, "%d,%lf,%lf,%lf", &mode, &a, &b, &c) == 4) cm = {mode, a, b, c};
+      int mode = 0; double a = 0, b = 0, c = 0, d = 0;
+      if (sscanf(e, "%d,%lf,%lf,%lf,%lf", &mode, &a, &b, &c, &d) == 5) cm = {mode, a, b, c, d};
     }
   }
   return cm;
 }
 
-int choose_bn(int Cout, long mtiles, int nkb, int sms, bool gelu) {
+double tile_main_loop(int nkb, int bn) {
+  const double mma = 12.0 * bn, l2 = (32768.0 + 256.0 * bn) / 42.0;
+  return nkb * (mma > l2 ? mma : l2);
+}
+// Staged epilogue (epilogue_staged) only where the register epilogue would not hide behind the other warpgroup's main loop: its
+// chunks take 33 KB of shared memory, a pipeline stage at BN = 32 and 96, which a long main loop feels and a hidden epilogue does
+// not repay.  The 10 % margin: at the crossover the staged epilogue measured slower (49152 x 2304 x 384, BN 128: main loop 56 k,
+// register epilogue 58 k clocks by the model; 5-9 % slower staged).
+bool stage_epilogue(bool vec2, int nkb, int bn) { return vec2 && tile_main_loop(nkb, bn) < 0.9 * cost_model().epi_reg * bn; }
+
+int choose_bn(int Cout, long mtiles, int nkb, int sms, bool gelu, bool vec2) {
   const CostModel& cm = cost_model();
   double best = 1e30; int best_bn = 32;
   for (int j = 1; j <= 16; ++j) {
@@ -432,8 +584,8 @@ int choose_bn(int Cout, long mtiles, int nkb, int sms, bool gelu) {
     if (bn > 128) continue;
     const long nt = (Cout + bn - 1) / bn;
     const long waves = (mtiles * nt + sms - 1) / sms;
-    const double mma = 12.0 * bn, l2 = (32768.0 + 256.0 * bn) / 42.0;
-    const double main_loop = nkb * (mma > l2 ? mma : l2), epi = (gelu ? cm.epi_gelu : cm.epi) * bn;
+    const double main_loop = tile_main_loop(nkb, bn);
+    const double epi = (stage_epilogue(vec2, nkb, bn) ? (gelu ? cm.epi_gelu : cm.epi) : cm.epi_reg) * bn;
     const double overlap = (main_loop + epi) / 2;
     const double tile = (cm.mode == 1 ? (main_loop > overlap ? main_loop : overlap) : main_loop + epi) + cm.fix;
     const double cost = waves * tile;
@@ -663,7 +815,8 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
   p.nkb = kdim / TC_BK;
   // ---- N tile: fixed by the row-stat layout for the vocabulary head, otherwise chosen per launch against wave quantisation
   const long mtiles = (long)p.N * p.tiles_y * p.tiles_x;
-  int BN = op.stat_max ? op.tc_bn : choose_bn(op.out.C, mtiles, p.nkb, num_sms, op.act == ACT_GELU);
+  fill_epi(p.e, op);
+  int BN = op.stat_max ? op.tc_bn : choose_bn(op.out.C, mtiles, p.nkb, num_sms, op.act == ACT_GELU, p.e.vec2 != 0);
   if (g_conv_force_bn && !op.stat_max) {
     MITB_CHECK(conv_tma_bn_candidate(op.out.C, g_conv_force_bn), "tma conv: BN %d is not a candidate N tile for Cout %d", g_conv_force_bn, op.out.C);
     BN = g_conv_force_bn;
@@ -672,7 +825,6 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
   p.npad = (op.out.C + BN - 1) / BN * BN;
   make_w_tmap(&p.tb_hi, stem ? op.w8h : padded_w ? op.whp : op.wh, kdim, op.tc_npad, BN);
   make_w_tmap(&p.tb_mid, stem ? op.w8m : padded_w ? op.wmp : op.wm, kdim, op.tc_npad, BN);
-  fill_epi(p.e, op);
   if (op.out_sv.valid()) {
     const SplitView& o = op.out_sv;
     MITB_CHECK(!op.out.planar && op.out.C % 4 == 0 && !op.stat_max && op.oy_mul == 1 && op.ox_mul == 1 && op.oy_add == 0 && op.ox_add == 0 &&
@@ -693,14 +845,18 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
     p.tile_need = tn;
   }
   const size_t stage_bytes = 2 * (size_t)TC_BM * 128 + 2 * (size_t)BN * 128;
-  int stages = (int)((227 * 1024 - 1024 - 256) / stage_bytes); if (stages > 6) stages = 6;
+  // the staged epilogue's chunks and row tables leave 4, 4, 3, 3 stages at BN 32, 64, 96, 128 (others: 5, 4, 4, 3)
+  p.staged = !op.stat_max && stage_epilogue(p.e.vec2 != 0, p.nkb, BN) ? 1 : 0;
+  const size_t epi_bytes = p.staged ? EPI_SMEM_BYTES : 0;
+  int stages = (int)((227 * 1024 - 1024 - 256 - epi_bytes) / stage_bytes); if (stages > 6) stages = 6;
   MITB_CHECK(stages >= 2, "tma conv: tile does not fit shared memory");
   p.stages = stages;
-  const size_t smem = stages * stage_bytes + 2 * stages * 8 + 1024;
+  p.bar_off = (int)(stages * stage_bytes + epi_bytes);
+  const size_t smem = stages * stage_bytes + epi_bytes + 2 * stages * 8 + 1024;
   const long total_tiles = mtiles * (p.npad / BN);
   const int grid = (int)(total_tiles < num_sms ? total_tiles : num_sms);      // persistent: one CTA per SM
   const int act_inst = op.stat_max ? ACT_NONE : (op.act == ACT_NONE || op.act == ACT_RELU || op.act == ACT_GELU || op.act == ACT_SILU) ? op.act : -1;
-  conv_trace(stem ? CK_STEM8 : CK_TMA, BN, 1, p.e.vec2, act_inst, reused);
+  conv_trace(stem ? CK_STEM8 : CK_TMA, BN, 1, p.e.vec2, act_inst, reused, p.staged ? (p.e.vec4 ? 4 : 2) : 0);
 #define MITB_TMA_LAUNCH(A)                                                              \
   switch (BN) {                                                                        \
     case 32: conv_tma_kernel<A, 32><<<grid, TM_THREADS, smem, st>>>(p); break;          \

@@ -127,12 +127,13 @@ struct ConvOp {
 void launch_conv(const ConvOp& op, cudaStream_t st);
 // Host-side record of what launch_conv() ran (test hook mitb_test_conv): null by default, and nothing is recorded then.
 enum ConvKernel { CK_SIMT = 1, CK_FEWOUT, CK_THIN, CK_GATHER, CK_GATHER_SPLITK, CK_TMA, CK_STEM8 };
-struct ConvTrace { int kernel = 0, bn = 0, splits = 1, vec2 = -1, tma_act = -2, split_reused = 0, convs = 0; };
+struct ConvTrace { int kernel = 0, bn = 0, splits = 1, vec2 = -1, tma_act = -2, split_reused = 0, convs = 0, staged = -1; };
 extern ConvTrace* g_conv_trace;
-inline void conv_trace(int kernel, int bn, int splits, int vec2, int tma_act, bool reused) {
+inline void conv_trace(int kernel, int bn, int splits, int vec2, int tma_act, bool reused, int staged = -1) {
   if (!g_conv_trace) return;
   ConvTrace& t = *g_conv_trace;
   t.kernel = kernel; t.bn = bn; t.splits = splits; t.vec2 = vec2; t.tma_act = tma_act; t.split_reused += reused ? 1 : 0; ++t.convs;
+  t.staged = staged;
 }
 extern int g_conv_force_bn;                // non-zero: the TMA kernel's N tile (must be one of choose_bn's candidates); test hook only
 bool conv_tma_bn_candidate(int Cout, int bn);

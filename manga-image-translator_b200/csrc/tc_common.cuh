@@ -16,6 +16,7 @@ struct EpiParams {
   const float* os_scale; const float* os_shift; int os_relu;  // consumer prologue applied before splitting
   float* partial; int npad;                                   // split-K: partial sums [splits][M][npad] (null: none)
   int vec2;                                                   // NHWC, even strides / offsets, 8-byte aligned operands, Cout even
+  int vec4;                                                   // vec2 with strides / offsets / Cout multiples of 4, 16-byte aligned (8 for os_hi / os_mid)
 };
 
 inline void fill_epi(EpiParams& e, const ConvOp& op) {
@@ -37,6 +38,11 @@ inline void fill_epi(EpiParams& e, const ConvOp& op) {
   e.vec2 = !op.out.planar && op.out.C % 2 == 0 && nhwc_ok(op.out) && nhwc_ok(op.add0) && nhwc_ok(op.add1) && al8(op.scale) && al8(op.shift) &&
            al8(op.mul1) && al8(op.os_scale) && al8(op.os_shift) && (!e.os_hi || ((e.os_pitch | e.os_coff) & 1) == 0) &&
            (!e.os_hi || (((uintptr_t)e.os_hi | (uintptr_t)e.os_mid) & 3) == 0);
+  auto al16 = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
+  auto nhwc_ok4 = [&](const View& v) { return !v.p || (((v.cs | v.coff) & 3) == 0 && al16(v.p)); };
+  e.vec4 = e.vec2 && op.out.C % 4 == 0 && nhwc_ok4(op.out) && nhwc_ok4(op.add0) && nhwc_ok4(op.add1) && al16(op.scale) && al16(op.shift) &&
+           al16(op.mul1) && al16(op.os_scale) && al16(op.os_shift) && (!e.os_hi || ((e.os_pitch | e.os_coff) & 3) == 0) &&
+           (!e.os_hi || (((uintptr_t)e.os_hi | (uintptr_t)e.os_mid) & 7) == 0);
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -235,6 +241,26 @@ __device__ __forceinline__ void stat_merge(float& am, float& as, int& ai, float 
   am = m;
 }
 
+// The fused elementwise chain of two adjacent columns, v = acc (+add0) ; v = v*scale+shift ; act ; *mul1 ; +add1, and the split of
+// its result into the consumer's bf16 hi / mid operands (after the consumer's prologue os_scale / os_shift / os_relu).  Every
+// two-column epilogue calls these, so the fp32 operations and their order, which the outputs' bits depend on, live in one place.
+template <int ACT>
+__device__ __forceinline__ void epi_chain2(const EpiParams& e, float& v0, float& v1, float2 a0, float2 sc, float2 sh, float2 m1, float2 a1) {
+  if (e.add0) { v0 += a0.x; v1 += a0.y; }
+  if (e.scale) { v0 *= sc.x; v1 *= sc.y; }
+  if (e.shift) { v0 += sh.x; v1 += sh.y; }
+  v0 = act_t<ACT>(v0, e.act); v1 = act_t<ACT>(v1, e.act);
+  if (e.mul1) { v0 *= m1.x; v1 *= m1.y; }
+  if (e.add1) { v0 += a1.x; v1 += a1.y; }
+}
+__device__ __forceinline__ void epi_split2(const EpiParams& e, float v0, float v1, float2 s, float2 t, uint32_t& hi, uint32_t& mid) {
+  if (e.os_scale) {
+    v0 = fmaf(v0, s.x, t.x); v1 = fmaf(v1, s.y, t.y);
+    if (e.os_relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+  }
+  split2(v0, v1, hi, mid);
+}
+
 // Epilogue of one 128 x BN output tile from the wgmma accumulator fragments.  Warp w of warpgroup g holds rows
 // 64 g + 16 (w % 4) + lane / 4 (registers 4j, 4j+1) and the row 8 below it (4j+2, 4j+3), columns 8 j + 2 (lane % 4) + {0, 1}:
 // a warp store covers 8 rows x 32 contiguous bytes, whole sectors.  rowpix(r, nimg, oy, ox) maps tile row r to its output pixel
@@ -335,21 +361,13 @@ __device__ __forceinline__ void epilogue_tile(const EpiParams& e, const float (&
           if (!kBothRows) load_row(h);
           if (!ok[h]) continue;
           float v0 = r[2 * h], v1 = r[2 * h + 1];
-          if (e.add0) { v0 += a0[h].x; v1 += a0[h].y; }
-          if (e.scale) { v0 *= sc.x; v1 *= sc.y; }
-          if (e.shift) { v0 += sh.x; v1 += sh.y; }
-          v0 = act_t<ACT>(v0, e.act); v1 = act_t<ACT>(v1, e.act);
-          if (e.mul1) { v0 *= m1.x; v1 *= m1.y; }
-          if (e.add1) { v0 += a1[h].x; v1 += a1[h].y; }
+          epi_chain2<ACT>(e, v0, v1, a0[h], sc, sh, m1, a1[h]);
           if (e.out) *reinterpret_cast<float2*>(e.out + (size_t)opix[h] * e.out_cs + e.out_coff + c) = make_float2(v0, v1);
           if (e.os_hi) {                     // producer -> consumer fusion: store the consumer's bf16 hi / mid operands directly
-            if (e.os_scale) {
-              const float2 s = __ldg(reinterpret_cast<const float2*>(e.os_scale + c)), t = __ldg(reinterpret_cast<const float2*>(e.os_shift + c));
-              v0 = fmaf(v0, s.x, t.x); v1 = fmaf(v1, s.y, t.y);
-              if (e.os_relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-            }
+            const float2 s = e.os_scale ? __ldg(reinterpret_cast<const float2*>(e.os_scale + c)) : z2;
+            const float2 t = e.os_scale ? __ldg(reinterpret_cast<const float2*>(e.os_shift + c)) : z2;
             uint32_t hh, mm;
-            split2(v0, v1, hh, mm);
+            epi_split2(e, v0, v1, s, t, hh, mm);
             const size_t so = (size_t)spix[h] * e.os_pitch + e.os_coff + c;
             *reinterpret_cast<uint32_t*>(e.os_hi + so) = hh;
             *reinterpret_cast<uint32_t*>(e.os_mid + so) = mm;

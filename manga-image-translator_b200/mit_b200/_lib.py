@@ -44,7 +44,7 @@ class MitbTestConvDesc(C.Structure):
 
 
 class MitbTestConvInfo(C.Structure):
-    _fields_ = _ints("kernel", "bn", "splits", "vec2", "tma_act", "split_reused", "convs", "reserved")
+    _fields_ = _ints("kernel", "bn", "splits", "vec2", "tma_act", "split_reused", "convs", "staged")
 
 
 class MitbError(RuntimeError):
