@@ -9,8 +9,8 @@
 // The vocabulary head uses the ROWSTAT epilogue: online (max, argmax, sum-exp) per row, so the [N,T,V]
 // logits never reach HBM (model_48px_ctc.py:460-461 computes log_softmax + max over them).
 //
-// This is the exact-fp32 path.  Layers that are large dense contractions are routed to the tcgen05 kernel in
-// conv_tc.cu by launch_conv(); this kernel remains the path for thin layers and the parity anchor of that one.
+// This is the exact-fp32 path.  Layers that are large dense contractions are routed to the wgmma kernels (conv_tma.cu,
+// conv_tc.cu) by conv_plan() (conv.cu); this kernel remains the path for thin layers and the parity anchor of those.
 #include <float.h>
 #include <limits.h>
 #include "mitb_internal.h"
@@ -19,8 +19,6 @@ namespace mitb {
 
 thread_local long* g_launch_counter = nullptr;
 unsigned long g_launch_epoch = 0;
-ConvTrace* g_conv_trace = nullptr;
-int g_conv_force_bn = 0;
 
 struct ConvKParams {
   const float* in; int N, H, W, in_cs, in_coff, Cin, in_planar;
@@ -34,24 +32,6 @@ struct ConvKParams {
   float* stat_max; float* stat_sum; int* stat_idx; int stat_ld;
   int M, K;
 };
-
-__device__ __forceinline__ float apply_act(float v, int act) {
-  switch (act) {
-    case ACT_RELU: return fmaxf(v, 0.f);
-    case ACT_GELU: return 0.5f * v * (1.f + erff(v * 0.70710678118654752440f));
-    case ACT_SILU: return v / (1.f + expf(-v));
-    case ACT_SIGMOID: return 1.f / (1.f + expf(-v));
-    case ACT_SIGMOID2: { float s = 1.f / (1.f + expf(-v)); return 1.f / (1.f + expf(-s)); }
-    case ACT_CLAMP01: return fminf(fmaxf(v, 0.f), 1.f);
-    default: return v;
-  }
-}
-
-__device__ __forceinline__ int reflect_idx(int i, int n) {
-  if (i < 0) i = -i;
-  if (i >= n) i = 2 * n - 2 - i;
-  return i;
-}
 
 constexpr int BM = 128, BK = 16, NT = 256, APAD = 4;
 
@@ -418,20 +398,11 @@ void launch_repack(float* dst, const float* src, int Cout, int Cin, int ntaps, c
 }
 
 
-
-bool conv_tc_supported(const ConvOp& op);            // conv_tc.cu
-int conv_tc_stat_blocks(const ConvOp& op);
-void launch_conv_tc(const ConvOp& op, cudaStream_t st);
-bool conv_thin_supported(const ConvOp& op);          // conv_thin.cu
-void launch_conv_thin(const ConvOp& op, cudaStream_t st);
-
-int conv_stat_blocks(const ConvOp& op) { return conv_tc_supported(op) ? conv_tc_stat_blocks(op) : (op.out.C + 127) / 128; }
-
 static void fill_params(const ConvOp& op, ConvKParams& p) {
   p.in = op.in.p; p.N = op.in.N; p.H = op.in.H; p.W = op.in.W; p.in_cs = op.in.cs; p.in_coff = op.in.coff;
   p.Cin = op.in.C; p.in_planar = op.in.planar;
-  p.w = op.w; p.ldw = op.ldw; p.ntaps = op.ntaps;
-  for (int t = 0; t < op.ntaps; ++t) { p.tdy[t] = op.tdy[t]; p.tdx[t] = op.tdx[t]; }
+  p.w = op.wt.w; p.ldw = op.wt.ldw; p.ntaps = op.wt.ntaps;
+  for (int t = 0; t < op.wt.ntaps; ++t) { p.tdy[t] = op.wt.tdy[t]; p.tdx[t] = op.wt.tdx[t]; }
   p.sy = op.sy; p.sx = op.sx; p.pad = op.pad; p.Ho = op.Ho; p.Wo = op.Wo;
   p.out = op.out.p; p.oH = op.out.H; p.oW = op.out.W; p.out_cs = op.out.cs; p.out_coff = op.out.coff;
   p.Cout = op.out.C; p.out_planar = op.out.planar;
@@ -441,55 +412,21 @@ static void fill_params(const ConvOp& op, ConvKParams& p) {
   p.add1 = op.add1.p; p.add1_cs = op.add1.cs; p.add1_coff = op.add1.coff; p.add1_planar = op.add1.planar;
   p.scale = op.scale; p.shift = op.shift; p.mul1 = op.mul1; p.act = op.act;
   p.stat_max = op.stat_max; p.stat_sum = op.stat_sum; p.stat_idx = op.stat_idx; p.stat_ld = op.stat_ld;
-  p.M = op.in.N * op.Ho * op.Wo; p.K = op.ntaps * op.in.C;
+  p.M = op.in.N * op.Ho * op.Wo; p.K = op.wt.ntaps * op.in.C;
 }
 
-void launch_conv(const ConvOp& op, cudaStream_t st) {
-  MITB_CHECK(op.ntaps >= 1 && op.ntaps <= kMaxTaps, "bad tap count %d", op.ntaps);
-  MITB_CHECK(op.in.N == op.out.N, "batch mismatch");
-  MITB_CHECK(op.ldw % 4 == 0 && op.ldw >= op.out.C, "bad ldw %d for Cout %d", op.ldw, op.out.C);
-  if (op.in.planar) {
-    MITB_CHECK(op.ntaps == 1 && op.sy == 1 && op.sx == 1 && op.tdy[0] == 0 && op.tdx[0] == 0 &&
-               op.Ho == op.in.H && op.Wo == op.in.W, "planar input supports 1x1 convs only");
-  } else {
-    MITB_CHECK(op.in.C % 4 == 0 && op.in.cs % 4 == 0 && op.in.coff % 4 == 0,
-               "NHWC conv input needs channel counts/offsets in multiples of 4 (C=%d cs=%d off=%d)", op.in.C, op.in.cs, op.in.coff);
-  }
-  if (op.pad == PAD_REFLECT) {
-    for (int t = 0; t < op.ntaps; ++t)
-      MITB_CHECK(-op.tdy[t] < op.in.H && -op.tdx[t] < op.in.W, "reflect padding wider than the image");
-  }
+// the fp32 kernels: the row-stat epilogue when op.stat_max is set, the thin-output kernel when conv_plan() picked CK_FEWOUT, else the
+// 128 x {64, 128} tile kernel
+void launch_conv_simt(const ConvOp& op, bool fewout, cudaStream_t st) {
   ConvKParams p; fill_params(op, p);
-  if (p.M == 0) return;
   const int Cout = op.out.C;
-  // algorithmic work of this launch: 2*M*K*Cout flops; bytes = input view + weights + output (+ fused residual reads)
-  if (op.seg2.sv.valid()) p.K += op.seg2.ntaps * op.seg2.C;          // second K segment of an operand-fused launch
-  const double flops = 2.0 * p.M * (double)p.K * Cout;
-  const double bytes = 4.0 * ((double)op.in.pixels() * op.in.C + (op.seg2.sv.valid() ? (double)op.in.pixels() * op.seg2.C : 0.0) + (double)p.K * Cout +
-                              (double)p.M * Cout * ((op.stat_max ? 0 : 1) + (op.add0.p ? 1 : 0) + (op.add1.p ? 1 : 0)));
-  if (conv_thin_supported(op)) {
-    // with an output-sparsity hint the executed work depends on the mask (device data): no flop figure is claimed for that class
-    const bool sparse = op.tile_mask || op.tile_mask_u8;
-    ProfScope ps(sparse ? "conv7_thin_sparse" : "conv7_thin", sparse ? 0.0 : flops, sparse ? 0.0 : bytes, st, p.M, p.K, Cout);
-    conv_trace(CK_THIN, 0, 1, -1, -2, false);
-    launch_conv_thin(op, st);
-    return;
-  }
-  if (conv_tc_supported(op)) {
-    // output-sparse launches (ConvOp::need_px): executed work depends on device data, so they form their own class without a flop claim
-    const bool sparse = op.need_px && !op.stat_max;
-    ProfScope ps(op.stat_max ? "conv_tc_rowstat" : sparse ? "conv_tc_sparse" : "conv_tc", sparse ? 0.0 : flops, sparse ? 0.0 : bytes, st, p.M, p.K, Cout);
-    launch_conv_tc(op, st);
-    return;
-  }
-  ProfScope ps(op.stat_max ? "conv_simt_rowstat" : (Cout <= 4 && !op.in.planar && op.ldw == 4) ? "conv_fewout" : "conv_simt", flops, bytes, st);
   if (op.stat_max) {
     MITB_CHECK(!op.in.planar, "row-stat epilogue expects NHWC input");
     dim3 grid((p.M + BM - 1) / BM, (Cout + 127) / 128);
     MITB_CHECK(op.stat_ld == (int)grid.y, "stat_ld must equal conv_stat_blocks(Cout)");
     conv_trace(CK_SIMT, 128, 1, -1, -2, false);
     conv_igemm_kernel<128, false, true><<<grid, NT, 0, st>>>(p);
-  } else if (Cout <= 4 && !op.in.planar && op.ldw == 4) {
+  } else if (fewout) {
     dim3 grid((p.M + 127) / 128);
     conv_trace(CK_FEWOUT, Cout, 1, -1, -2, false);
     switch (Cout) {

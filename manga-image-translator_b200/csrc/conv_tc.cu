@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             const int iy0 = ryx[i] >> 16, ix0 = ryx[i] & 0xffff;
             int iy = iy0 + dy, ix = ix0 + dx;
             bool inb = true;
-            if (p.pad == PAD_REFLECT) { iy = reflect_tc(iy, p.H); ix = reflect_tc(ix, p.W); }
+            if (p.pad == PAD_REFLECT) { iy = reflect_idx(iy, p.H); ix = reflect_idx(ix, p.W); }
             else inb = (iy >= 0) & (iy < p.H) & (ix >= 0) & (ix < p.W);
             if (inb) {
               v[i] = __ldg(reinterpret_cast<const float4*>(p.in + (roff[i] + (uint32_t)(((iy - iy0) * p.W + (ix - ix0)) * p.in_cs + ci))));
@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const __grid_constan
       if (p.add0) x += p.add0_planar ? p.add0[((size_t)nimg * p.add0_cs + p.add0_coff + c) * oplane + opl_pix] : p.add0[opix * p.add0_cs + p.add0_coff + c];
       if (p.scale) x *= __ldg(p.scale + c);
       if (p.shift) x += __ldg(p.shift + c);
-      x = apply_act_tc(x, p.act);
+      x = apply_act(x, p.act);
       if (p.mul1) x *= __ldg(p.mul1 + c);
       if (p.add1) x += p.add1_planar ? p.add1[((size_t)nimg * p.add1_cs + p.add1_coff + c) * oplane + opl_pix] : p.add1[opix * p.add1_cs + p.add1_coff + c];
       if (p.out_planar) p.out[((size_t)nimg * p.out_cs + p.out_coff + c) * oplane + opl_pix] = x;
@@ -302,33 +302,6 @@ static bool g_tc_enabled = true;
 void conv_tc_set_enabled(bool on) { g_tc_enabled = on; }
 bool conv_tc_enabled() { return g_tc_enabled; }
 
-// TMA descriptor of a K-major bf16 weight matrix [npad][kpad]: box = 64 k (128 bytes, SWIZZLE_128B) x BN rows.
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr; cudaDriverEntryPointQueryResult q;
-    CUDA_OK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q));
-    MITB_CHECK(p && q == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available in this driver");
-    fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-static void make_weight_tmap(TmaDesc* out, const uint16_t* base, int kpad, int npad, int bn) {
-  CUtensorMap m;
-  const cuuint64_t gdim[2] = {(cuuint64_t)kpad, (cuuint64_t)npad};
-  const cuuint64_t gstride[1] = {(cuuint64_t)kpad * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)bn};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)base, gdim, gstride, box, estr,
-                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  MITB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for [%d x %d] box %d", (int)r, npad, kpad, bn);
-  memcpy(out, &m, sizeof(m));
-}
-
 // fp32 K-major [(ky*kw+kx)*4 + c][ldw] -> bf16 hi/mid [npad][kh*64] with k = ky*64 + kx*8 + c (zero elsewhere): Cin = 4 stems
 __global__ void split_weights_stem8_kernel(const float* w, int kh, int kw, int Cout, int ldw, uint16_t* wh, uint16_t* wm, int npad) {
   const int kp = kh * 64;
@@ -356,8 +329,6 @@ void conv_tc_prepare(ConvW& cw, DevBlob& blob, cudaStream_t st) {
   split_weights_kernel<<<blocks, 256, 0, st>>>(cw.w, K, cw.Cout, cw.ldw, wh, wm, cw.tc_kpad, cw.tc_npad);
   CUDA_OK(cudaGetLastError());
   cw.wh = wh; cw.wm = wm;
-  make_weight_tmap(&cw.tmh, wh, cw.tc_kpad, cw.tc_npad, bn);
-  make_weight_tmap(&cw.tmm, wm, cw.tc_kpad, cw.tc_npad, bn);
   if (cw.Cin % 64 != 0 && cw.Cin % 8 == 0 && cw.Cin >= 16) {
     // the TMA-fed kernel consumes K blocks of 64 channels of one tap: give it a copy with each tap padded to a multiple of 64
     const int cp = (cw.Cin + 63) / 64 * 64;
@@ -387,59 +358,38 @@ void conv_tc_prepare(ConvW& cw, DevBlob& blob, cudaStream_t st) {
   }
 }
 
-int conv_tc_stat_blocks(const ConvOp& op) { return 2 * (op.tc_npad / op.tc_bn); }   // two column halves per N tile
-
 bool conv_tc_supported(const ConvOp& op) {
-  if (!g_tc_enabled || !op.wh || !op.wm) return false;
-  const int K = op.ntaps * op.in.C;
+  if (!g_tc_enabled || !op.wt.wh || !op.wt.wm) return false;
+  const int K = op.wt.ntaps * op.in.C;
   if (K < 32) return false;
-  if (op.in.planar) return op.ntaps == 1;
+  if (op.in.planar) return op.wt.ntaps == 1;
   return op.in.C % 4 == 0 && op.in.cs % 4 == 0 && op.in.coff % 4 == 0;
 }
 
-bool conv_tma_supported(const ConvOp& op);     // conv_tma.cu
-void launch_conv_tma(const ConvOp& op, cudaStream_t st);
-bool conv_stem8_supported(const ConvOp& op);
-void launch_conv_stem8(const ConvOp& op, cudaStream_t st);
-
-static bool tma_dispatch(const ConvOp& op) {
-  if (!conv_tma_supported(op)) return false;
-  if (op.in_sv.valid() || op.out_sv.valid() || op.seg2.sv.valid()) return true;   // operand-fused ops exist only on the TMA path
-  // TMA-fed kernel unless the layer is so small that it needs split-K
-  const int sms = device_sm_count();
-  const long Mrows = (long)op.in.N * op.Ho * op.Wo;
-  const long tiles = ((Mrows + TC_BM - 1) / TC_BM) * (op.tc_npad / op.tc_bn);
-  const bool would_split = !op.stat_max && tiles * 2 <= sms && op.tc_kpad / TC_BK >= 16;
-  return !would_split;
-}
-bool conv_tma_capable(const ConvOp& op) { return op.out.C > 4 && conv_tc_supported(op) && conv_tma_supported(op); }
-bool conv_uses_tma(const ConvOp& op) { return op.out.C > 4 && conv_tc_supported(op) && tma_dispatch(op); }
-
-void launch_conv_tc(const ConvOp& op, cudaStream_t st) {
-  if (conv_stem8_supported(op)) { launch_conv_stem8(op, st); return; }
-  if (tma_dispatch(op)) { launch_conv_tma(op, st); return; }
-  MITB_CHECK(!op.in_sv.valid() && !op.out_sv.valid() && !op.seg2.sv.valid(), "conv: operand-fused ops must run on the TMA path");
+// the register-gather kernel, split-K over `splits` (conv_plan()) with a second reduce launch
+void launch_conv_tc(const ConvOp& op, int splits, cudaStream_t st) {
+  const ConvW& w = op.wt;
   TcParams p;
   p.in = op.in.p; p.N = op.in.N; p.H = op.in.H; p.W = op.in.W; p.in_cs = op.in.cs; p.in_coff = op.in.coff; p.Cin = op.in.C;
   p.in_planar = op.in.planar;
-  static_assert(sizeof(CUtensorMap) == sizeof(TmaDesc), "TmaDesc must mirror CUtensorMap");
-  memcpy(&p.tmh, &op.tmh, sizeof(CUtensorMap)); memcpy(&p.tmm, &op.tmm, sizeof(CUtensorMap));
-  p.kpad = op.tc_kpad; p.npad = op.tc_npad;
-  p.ntaps = op.ntaps;
+  make_w_tmap(&p.tmh, w.wh, w.tc_kpad, w.tc_npad, w.tc_bn);
+  make_w_tmap(&p.tmm, w.wm, w.tc_kpad, w.tc_npad, w.tc_bn);
+  p.kpad = w.tc_kpad; p.npad = w.tc_npad;
+  p.ntaps = w.ntaps;
   p.tmin_dy = p.tmin_dx = 127; p.tmax_dy = p.tmax_dx = -127;
-  for (int t = 0; t < op.ntaps; ++t) {
-    p.tdy[t] = op.tdy[t]; p.tdx[t] = op.tdx[t];
-    if (op.tdy[t] < p.tmin_dy) p.tmin_dy = op.tdy[t];
-    if (op.tdy[t] > p.tmax_dy) p.tmax_dy = op.tdy[t];
-    if (op.tdx[t] < p.tmin_dx) p.tmin_dx = op.tdx[t];
-    if (op.tdx[t] > p.tmax_dx) p.tmax_dx = op.tdx[t];
+  for (int t = 0; t < w.ntaps; ++t) {
+    p.tdy[t] = w.tdy[t]; p.tdx[t] = w.tdx[t];
+    if (w.tdy[t] < p.tmin_dy) p.tmin_dy = w.tdy[t];
+    if (w.tdy[t] > p.tmax_dy) p.tmax_dy = w.tdy[t];
+    if (w.tdx[t] < p.tmin_dx) p.tmin_dx = w.tdx[t];
+    if (w.tdx[t] > p.tmax_dx) p.tmax_dx = w.tdx[t];
   }
   p.sy = op.sy; p.sx = op.sx; p.pad = op.pad; p.Ho = op.Ho; p.Wo = op.Wo;
   p.in_scale = op.in_scale; p.in_shift = op.in_shift; p.in_relu = op.in_relu;
   fill_epi(p.e, op);
-  MITB_CHECK(!op.stat_max || op.stat_ld == 2 * (op.tc_npad / op.tc_bn), "tc conv: stat_ld must equal conv_stat_blocks(op)");
-  p.M = op.in.N * op.Ho * op.Wo; p.K = op.ntaps * op.in.C;
-  const int BN = op.tc_bn;
+  MITB_CHECK(!op.stat_max || op.stat_ld == 2 * (w.tc_npad / w.tc_bn), "tc conv: stat_ld must equal conv_stat_blocks(op)");
+  p.M = op.in.N * op.Ho * op.Wo; p.K = w.ntaps * op.in.C;
+  const int BN = w.tc_bn;
   MITB_CHECK(BN >= 32 && BN <= 128 && BN % 32 == 0, "tc conv: bad BN %d", BN);
   MITB_CHECK(p.in_planar || p.Cin % 4 == 0, "tc conv: Cin must be a multiple of 4");
   MITB_CHECK((size_t)op.in.pixels() * op.in.cs < (size_t)1 << 31, "tc conv: input tensor too large for 32-bit element offsets");
@@ -453,15 +403,7 @@ void launch_conv_tc(const ConvOp& op, cudaStream_t st) {
     CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   }
-  const int mt = (p.M + TC_BM - 1) / TC_BM, nt = p.npad / BN;
-  // split-K for layers whose tile count cannot fill the SMs (deep, spatially tiny layers of the DBNet decoder)
-  const int tiles = mt * nt, nkb = p.kpad / TC_BK;
-  int splits = 1;
-  if (!op.stat_max && tiles * 2 <= num_sms && nkb >= 16) {
-    splits = num_sms / tiles;
-    if (splits > nkb / 4) splits = nkb / 4;
-    if (splits < 1) splits = 1;
-  }
+  const int tiles = ((p.M + TC_BM - 1) / TC_BM) * (p.npad / BN);
   p.splits = splits;
   if (splits > 1) {
     const size_t need = (size_t)splits * p.M * p.npad * sizeof(float);

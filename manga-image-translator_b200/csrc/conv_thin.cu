@@ -151,25 +151,26 @@ __global__ void __launch_bounds__(256, 2) conv7_thin_kernel(const ThinParams p) 
 }  // namespace
 
 bool conv_thin_supported(const ConvOp& op) {
-  if (op.in.planar || op.stat_max || op.ntaps != KS * KS || op.out.C > 4 || op.ldw != 4) return false;
+  if (op.in.planar || op.stat_max || op.wt.ntaps != KS * KS || op.out.C > 4 || op.wt.ldw != 4) return false;
   if (op.sy != 1 || op.sx != 1 || op.in.C % CCH != 0 || op.in.cs % 4 != 0 || op.in.coff % 4 != 0) return false;
   if (op.Ho != op.in.H || op.Wo != op.in.W || op.oy_mul != 1 || op.ox_mul != 1 || op.oy_add || op.ox_add) return false;
   if (op.in_scale || op.add0.p || op.add1.p || op.scale || op.mul1) return false;
   if (op.act != ACT_NONE && op.act != ACT_RELU && op.act != ACT_SILU && op.act != ACT_SIGMOID) return false;
-  for (int t = 0; t < op.ntaps; ++t)
-    if (op.tdy[t] != t / KS - HALO || op.tdx[t] != t % KS - HALO) return false;
+  for (int t = 0; t < op.wt.ntaps; ++t)
+    if (op.wt.tdy[t] != t / KS - HALO || op.wt.tdx[t] != t % KS - HALO) return false;
   return op.in.H >= 4 && op.in.W >= 4;
 }
 
 void launch_conv_thin(const ConvOp& op, cudaStream_t st) {
   ThinParams p;
   p.in = op.in.p; p.N = op.in.N; p.H = op.in.H; p.W = op.in.W; p.in_cs = op.in.cs; p.in_coff = op.in.coff; p.Cin = op.in.C;
-  p.w = op.w; p.out = op.out.p; p.out_cs = op.out.cs; p.out_coff = op.out.coff; p.Cout = op.out.C; p.out_planar = op.out.planar;
+  p.w = op.wt.w; p.out = op.out.p; p.out_cs = op.out.cs; p.out_coff = op.out.coff; p.Cout = op.out.C; p.out_planar = op.out.planar;
   p.shift = op.shift; p.act = op.act; p.pad = op.pad; p.tile_mask = op.tile_mask; p.tile_mask_u8 = op.tile_mask_u8;
   const size_t smem = (size_t)(CCH * SH * SW + CCH * KS * KS * 4) * sizeof(float);
   static PerDeviceOnce attr;
   if (attr.first()) CUDA_OK(cudaFuncSetAttribute(conv7_thin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   dim3 grid((p.W + TW - 1) / TW, (p.H + TH - 1) / TH, p.N);
+  conv_trace(CK_THIN, 0, 1, -1, -2, false);
   conv7_thin_kernel<<<grid, 256, smem, st>>>(p);
   count_launch();
   CUDA_OK(cudaGetLastError());

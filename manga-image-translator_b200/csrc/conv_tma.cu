@@ -112,7 +112,7 @@ template <> __device__ __forceinline__ void st_bf16_w<2>(uint16_t* q, const uint
 
 // The fused chain of one 128 x BN tile: acc0 holds rows 0-63, acc1 rows 64-127 (fragment layout of epilogue_tile; `row` is this
 // thread's first row); both are consumed.  rowpix(r, ...) as in epilogue_tile; rowm(r) is the tile row's index in the logical output
-// grid, which is the pixel index of out / add0 / add1 whenever there is a split output (tma_launch admits out_sv only on the conv's
+// grid, which is the pixel index of out / add0 / add1 whenever there is a split output (launch_conv_tma admits out_sv only on the conv's
 // own grid), so the row table needs one entry per row.  `bar` is this warpgroup's named barrier.
 template <int ACT, int BN, int W, class RowPix, class RowM>
 __device__ __forceinline__ void epilogue_staged(const EpiParams& e, float (&acc0)[BN / 2], float (&acc1)[BN / 2], int row, int n0, float* chunk,
@@ -400,7 +400,7 @@ __global__ void __launch_bounds__(256) split_pad_kernel(const SplitParams q) {
     else { pix = i / c8n; c8 = (int)(i - pix * c8n); }                        // channel fastest: NHWC reads coalesced
     const int x = (int)(pix % q.Wp); const long r = pix / q.Wp;
     const int y = (int)(r % q.Hp), n = (int)(r / q.Hp);
-    const int sy = reflect_tc(y - q.pt, q.H), sx = reflect_tc(x - q.pl, q.W);
+    const int sy = reflect_idx(y - q.pt, q.H), sx = reflect_idx(x - q.pl, q.W);
     const int c0 = c8 * 8;
     float v[8];
     if (q.planar) {
@@ -440,7 +440,7 @@ __global__ void __launch_bounds__(256) split_halo_kernel(uint16_t* hi, uint16_t*
     int y, x;
     if (j < rows_h) { const int r = (int)(j / Wp); x = (int)(j - (long)r * Wp); y = r < pt ? r : r + H; }
     else { const long k = j - rows_h; const int r = (int)(k / (Wp - W)); const int xx = (int)(k - (long)r * (Wp - W)); y = pt + r; x = xx < pl ? xx : xx + W; }
-    const int sy = reflect_tc(y - pt, H) + pt, sx = reflect_tc(x - pl, W) + pl;
+    const int sy = reflect_idx(y - pt, H) + pt, sx = reflect_idx(x - pl, W) + pl;
     const size_t so = ((size_t)(n * Hp + sy) * Wp + sx) * pitch + coff + c8 * 8;
     const size_t dst_o = ((size_t)(n * Hp + y) * Wp + x) * pitch + coff + c8 * 8;
     *reinterpret_cast<uint4*>(hi + dst_o) = *reinterpret_cast<const uint4*>(hi + so);
@@ -458,7 +458,7 @@ __global__ void __launch_bounds__(256) split_stem8_kernel(const float* in, int N
     const int y = (int)(r % Hp), n = (int)(r / Hp);
     int sy = y - pt, sx = x - pl;
     bool ok = true;
-    if (reflect) { sy = reflect_tc(sy, H); sx = reflect_tc(sx, W); ok = sx >= 0 && sx < W && sy >= 0 && sy < H; }
+    if (reflect) { sy = reflect_idx(sy, H); sx = reflect_idx(sx, W); ok = sx >= 0 && sx < W && sy >= 0 && sy < H; }
     else ok = sy >= 0 && sy < H && sx >= 0 && sx < W;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (ok) v = __ldg(reinterpret_cast<const float4*>(in + ((size_t)(n * H + sy) * W + sx) * cs + coff));
@@ -531,18 +531,6 @@ bool make_stem_tmap(CUtensorMap* m, const uint16_t* base, int N, int Hp, int Wp,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// weight map over bf16 [rows][kdim] K-major: box {64 k, bn}; rows beyond `rows` are zero filled
-void make_w_tmap(CUtensorMap* m, const uint16_t* base, int kdim, int rows, int bn) {
-  const cuuint64_t gdim[2] = {(cuuint64_t)kdim, (cuuint64_t)rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)kdim * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)bn};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = encode_fn()(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)base, gdim, gstride, box, estr,
-                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  MITB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for weights [%d x %d] box %d", (int)r, rows, kdim, bn);
-}
-
 // N tile width: minimise waves x tile time.  Main loop = K blocks x max(tensor floor, operand bytes over the SM's share of L2
 // bandwidth); candidates split Cout into j equal tiles rounded up to 32 (the wgmma widths instantiated, at most 128).  Tensor
 // floor: 3 x 128 x bn x 64 bf16 MACs per K block at the H100 SXM data-sheet dense bf16 rate (~2048 MAC per clock per SM) =
@@ -613,6 +601,17 @@ void conv_halo(const int8_t* tdy, const int8_t* tdx, int ntaps, int pad, int H, 
 
 }  // namespace
 
+void make_w_tmap(CUtensorMap* m, const uint16_t* base, int kdim, int rows, int bn) {
+  const cuuint64_t gdim[2] = {(cuuint64_t)kdim, (cuuint64_t)rows};
+  const cuuint64_t gstride[1] = {(cuuint64_t)kdim * 2};
+  const cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)bn};
+  const cuuint32_t estr[2] = {1, 1};
+  const CUresult r = encode_fn()(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)base, gdim, gstride, box, estr,
+                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  MITB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for weights [%d x %d] box %d", (int)r, rows, kdim, bn);
+}
+
 void conv_tma_set_enabled(bool on) { g_tma_enabled = on; }
 bool conv_tma_enabled() { return g_tma_enabled; }
 bool conv_tma_bn_candidate(int Cout, int bn) {
@@ -653,14 +652,14 @@ void launch_split_halo(const SplitView& sv, int coff, int C, cudaStream_t st) {
 bool conv_tma_supported(const ConvOp& op) {
   static int env = -1;
   if (env < 0) { const char* e = getenv("MITB_NO_TMA_CONV"); env = (e && atoi(e)) ? 0 : 1; }
-  if (!g_tma_enabled || !env || !op.wh || !op.wm) return false;
+  if (!g_tma_enabled || !env || !op.wt.wh || !op.wt.wm) return false;
   if (op.sy < 1 || op.sy > 2 || op.sx < 1 || op.sx > 2) return false;
   const int C = op.in.C;
-  if (C % 64 == 0) { if (!op.seg2.sv.valid() && op.tc_kpad != op.ntaps * C) return false; }   // main copy is already in (tap, 64-channel block) order
-  else if (!(op.whp && op.wmp && op.tc_cp >= C)) return false;             // needs the per-tap padded copy (Cin % 8 == 0, >= 16)
+  if (C % 64 == 0) { if (!op.seg2.sv.valid() && op.wt.tc_kpad != op.wt.ntaps * C) return false; }   // main copy is already in (tap, 64-channel block) order
+  else if (!(op.wt.whp && op.wt.wmp && op.wt.tc_cp >= C)) return false;             // needs the per-tap padded copy (Cin % 8 == 0, >= 16)
   if (!op.in_sv.valid()) {
     if (!op.in.planar && (op.in.cs % 4 != 0 || op.in.coff % 4 != 0)) return false;
-    if (op.in.planar && op.ntaps != 1) return false;
+    if (op.in.planar && op.wt.ntaps != 1) return false;
   }
   const long M = (long)op.in.N * op.Ho * op.Wo;
   if (M < 128) return false;
@@ -672,26 +671,22 @@ static bool g_stem_map_failed = false;       // the driver refused the overlappi
 bool conv_stem8_supported(const ConvOp& op) {
   static int env = -1;
   if (env < 0) { const char* e = getenv("MITB_NO_STEM8"); env = (e && atoi(e)) ? 0 : 1; }
-  if (!g_tma_enabled || !env || g_stem_map_failed || !op.w8h || !op.w8m) return false;
+  if (!g_tma_enabled || !env || g_stem_map_failed || !op.wt.w8h || !op.wt.w8m) return false;
   // strides 1 and 2 only (the ConvNeXt 4x4 s4 stem keeps the gather kernel)
-  if (op.in.C != 4 || op.in.planar || op.sx != op.sy || (op.sx != 1 && op.sx != 2) || op.ntaps != op.w8_kh * op.w8_kw) return false;
+  if (op.in.C != 4 || op.in.planar || op.sx != op.sy || (op.sx != 1 && op.sx != 2) || op.wt.ntaps != op.wt.w8_kh * op.wt.w8_kw) return false;
   if ((op.in.cs | op.in.coff) & 3) return false;
   if (op.in_sv.valid() || op.seg2.sv.valid() || op.stat_max || op.out.C <= 4) return false;
-  if (op.pad == PAD_REFLECT && (-op.tdy[0] >= op.in.H || -op.tdx[0] >= op.in.W)) return false;
+  if (op.pad == PAD_REFLECT && (-op.wt.tdy[0] >= op.in.H || -op.wt.tdx[0] >= op.in.W)) return false;
   return (long)op.in.N * op.Ho * op.Wo >= 128;
 }
 
-static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem);
-void launch_conv_tma(const ConvOp& op, cudaStream_t st) { tma_launch(op, st, false); }
-void launch_conv_stem8(const ConvOp& op, cudaStream_t st) { tma_launch(op, st, true); }
-
-static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
+void launch_conv_tma(const ConvOp& op, bool stem, cudaStream_t st) {
   const int C = op.in.C, N = op.in.N, H = op.in.H, W = op.in.W;
   const bool padded_w = !stem && C % 64 != 0;
   const int cblks = stem ? 1 : (C + TC_BK - 1) / TC_BK;              // K blocks per tap; channels >= C arrive as zeros (TMA bounds)
   int pt, pb, pl, pr;
-  conv_halo(op.tdy, op.tdx, op.ntaps, stem ? PAD_REFLECT : op.pad, H, W, op.Ho, op.Wo, op.sy, op.sx, pt, pb, pl, pr);
-  if (stem) pr += 8 - op.w8_kw;                                       // every window is 8 pixels wide (the extra taps have zero weights)
+  conv_halo(op.wt.tdy, op.wt.tdx, op.wt.ntaps, stem ? PAD_REFLECT : op.pad, H, W, op.Ho, op.Wo, op.sy, op.sx, pt, pb, pl, pr);
+  if (stem) pr += 8 - op.wt.w8_kw;                                       // every window is 8 pixels wide (the extra taps have zero weights)
   SplitView sv; int sv_coff = 0;
   int dev = 0; CUDA_OK(cudaGetDevice(&dev));
   // the split cache below: remembers which tensor the per-device scratch currently holds
@@ -711,7 +706,7 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
     MITB_CHECK(sv.pt >= pt && sv.pl >= pl && sv.Hp - sv.H - sv.pt >= pb && sv.Wp - sv.W - sv.pl >= pr, "tma conv: in_sv halo too small");
     if (op.pad != PAD_REFLECT && (sv.Hp != sv.H || sv.Wp != sv.W)) {      // zero padding over a halo'd tensor: only if no tap leaves the image
       int zt, zb, zl, zr;
-      conv_halo(op.tdy, op.tdx, op.ntaps, PAD_REFLECT, H, W, op.Ho, op.Wo, op.sy, op.sx, zt, zb, zl, zr);
+      conv_halo(op.wt.tdy, op.wt.tdx, op.wt.ntaps, PAD_REFLECT, H, W, op.Ho, op.Wo, op.sy, op.sx, zt, zb, zl, zr);
       MITB_CHECK(zt == 0 && zb == 0 && zl == 0 && zr == 0, "tma conv: zero padding needs a halo-free in_sv");
     }
     MITB_CHECK(!op.in_scale, "tma conv: in_sv carries its prologue already");
@@ -763,11 +758,11 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
   memset(&p, 0, sizeof(p));
   const bool two = op.seg2.sv.valid();
   p.nseg = two ? 2 : 1;
-  p.seg[0].ntaps = stem ? op.w8_kh : op.ntaps; p.seg[0].cblks = cblks; p.seg[0].c0 = sv_coff;
-  if (stem) for (int t = 0; t < op.w8_kh; ++t) { p.seg[0].tdy[t] = (int8_t)(op.tdy[t * op.w8_kw] + sv.pt); p.seg[0].tdx[t] = (int8_t)(op.tdx[0] + sv.pl); }
-  else for (int t = 0; t < op.ntaps; ++t) { p.seg[0].tdy[t] = (int8_t)(op.tdy[t] + sv.pt); p.seg[0].tdx[t] = (int8_t)(op.tdx[t] + sv.pl); }
+  p.seg[0].ntaps = stem ? op.wt.w8_kh : op.wt.ntaps; p.seg[0].cblks = cblks; p.seg[0].c0 = sv_coff;
+  if (stem) for (int t = 0; t < op.wt.w8_kh; ++t) { p.seg[0].tdy[t] = (int8_t)(op.wt.tdy[t * op.wt.w8_kw] + sv.pt); p.seg[0].tdx[t] = (int8_t)(op.wt.tdx[0] + sv.pl); }
+  else for (int t = 0; t < op.wt.ntaps; ++t) { p.seg[0].tdy[t] = (int8_t)(op.wt.tdy[t] + sv.pt); p.seg[0].tdx[t] = (int8_t)(op.wt.tdx[t] + sv.pl); }
   p.N = N; p.Ho = op.Ho; p.Wo = op.Wo; p.M = N * op.Ho * op.Wo; p.sy = op.sy; p.sx = op.sx;
-  const bool lin = !stem && !two && op.ntaps == 1 && op.Ho == H && op.Wo == W && op.sy == 1 && op.sx == 1 && op.tdy[0] == 0 && op.tdx[0] == 0 &&
+  const bool lin = !stem && !two && op.wt.ntaps == 1 && op.Ho == H && op.Wo == W && op.sy == 1 && op.sx == 1 && op.wt.tdy[0] == 0 && op.wt.tdx[0] == 0 &&
                    sv.Hp == H && sv.Wp == W;
   p.lin = lin ? 1 : 0;                                              // 1x1: flattened [pixels][C] matrix
   int bw, bh;
@@ -793,7 +788,7 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
     }
   } else if (lin) { make_act_tmap(&p.seg[0].ta_hi, sv.hi, 1, 1, N * sv.Hp * sv.Wp, sv.C, bw, bh, 1, 1); make_act_tmap(&p.seg[0].ta_mid, sv.mid, 1, 1, N * sv.Hp * sv.Wp, sv.C, bw, bh, 1, 1); }
   else { make_act_tmap(&p.seg[0].ta_hi, sv.hi, N, sv.Hp, sv.Wp, sv.C, bw, bh, op.sx, op.sy); make_act_tmap(&p.seg[0].ta_mid, sv.mid, N, sv.Hp, sv.Wp, sv.C, bw, bh, op.sx, op.sy); }
-  int kdim = (stem ? op.w8_kh : op.ntaps) * cblks * TC_BK;
+  int kdim = (stem ? op.wt.w8_kh : op.wt.ntaps) * cblks * TC_BK;
   if (two) {
     const ConvOp::Seg2& s2 = op.seg2;
     MITB_CHECK(!padded_w && s2.C % 64 == 0 && s2.ntaps >= 1 && s2.sv.N == N && s2.sv.H == op.Ho && s2.sv.W == op.Wo && op.sy == 1 && op.sx == 1 &&
@@ -810,21 +805,21 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
     make_act_tmap(&p.seg[1].ta_hi, s2.sv.hi, N, s2.sv.Hp, s2.sv.Wp, s2.sv.C, bw, bh, 1, 1);
     make_act_tmap(&p.seg[1].ta_mid, s2.sv.mid, N, s2.sv.Hp, s2.sv.Wp, s2.sv.C, bw, bh, 1, 1);
     kdim += s2.ntaps * s2.C;
-    MITB_CHECK(op.tc_kpad == kdim, "tma conv: merged weight has K %d, segments need %d", op.tc_kpad, kdim);
+    MITB_CHECK(op.wt.tc_kpad == kdim, "tma conv: merged weight has K %d, segments need %d", op.wt.tc_kpad, kdim);
   }
   p.nkb = kdim / TC_BK;
   // ---- N tile: fixed by the row-stat layout for the vocabulary head, otherwise chosen per launch against wave quantisation
   const long mtiles = (long)p.N * p.tiles_y * p.tiles_x;
   fill_epi(p.e, op);
-  int BN = op.stat_max ? op.tc_bn : choose_bn(op.out.C, mtiles, p.nkb, num_sms, op.act == ACT_GELU, p.e.vec2 != 0);
+  int BN = op.stat_max ? op.wt.tc_bn : choose_bn(op.out.C, mtiles, p.nkb, num_sms, op.act == ACT_GELU, p.e.vec2 != 0);
   if (g_conv_force_bn && !op.stat_max) {
     MITB_CHECK(conv_tma_bn_candidate(op.out.C, g_conv_force_bn), "tma conv: BN %d is not a candidate N tile for Cout %d", g_conv_force_bn, op.out.C);
     BN = g_conv_force_bn;
   }
   MITB_CHECK(BN >= 32 && BN <= 128 && BN % 32 == 0, "tma conv: bad BN %d", BN);
   p.npad = (op.out.C + BN - 1) / BN * BN;
-  make_w_tmap(&p.tb_hi, stem ? op.w8h : padded_w ? op.whp : op.wh, kdim, op.tc_npad, BN);
-  make_w_tmap(&p.tb_mid, stem ? op.w8m : padded_w ? op.wmp : op.wm, kdim, op.tc_npad, BN);
+  make_w_tmap(&p.tb_hi, stem ? op.wt.w8h : padded_w ? op.wt.whp : op.wt.wh, kdim, op.wt.tc_npad, BN);
+  make_w_tmap(&p.tb_mid, stem ? op.wt.w8m : padded_w ? op.wt.wmp : op.wt.wm, kdim, op.wt.tc_npad, BN);
   if (op.out_sv.valid()) {
     const SplitView& o = op.out_sv;
     MITB_CHECK(!op.out.planar && op.out.C % 4 == 0 && !op.stat_max && op.oy_mul == 1 && op.ox_mul == 1 && op.oy_add == 0 && op.ox_add == 0 &&
@@ -835,7 +830,7 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
                "tma conv: out_sv needs an NHWC output on the conv's own pixel grid");
     if (!op.out.p) { p.e.oH = op.Ho; p.e.oW = op.Wo; }
   } else MITB_CHECK(op.out.p || op.stat_max, "tma conv: no output");
-  MITB_CHECK(!op.stat_max || op.stat_ld == 2 * (op.tc_npad / op.tc_bn), "tma conv: stat_ld must equal conv_stat_blocks(op)");
+  MITB_CHECK(!op.stat_max || op.stat_ld == 2 * (op.wt.tc_npad / op.wt.tc_bn), "tma conv: stat_ld must equal conv_stat_blocks(op)");
   if (op.need_px && !op.stat_max) {
     // reduce the pixel-level hint to this launch's tile grid (one tiny launch; the scratch is per device and stream ordered)
     static DeviceScratch g_need;
@@ -882,7 +877,7 @@ static void tma_launch(const ConvOp& op, cudaStream_t st, bool stem) {
     CUDA_OK(cudaMemcpyFromSymbol(ph, g_conv_phases, sizeof(ph)));
     const unsigned long long zero[5] = {0, 0, 0, 0, 0};
     CUDA_OK(cudaMemcpyToSymbol(g_conv_phases, zero, sizeof(zero)));
-    const int K = op.ntaps * C + (two ? op.seg2.ntaps * op.seg2.C : 0);      // the GEMM shape tools/layer_times.py reports
+    const int K = op.wt.ntaps * C + (two ? op.seg2.ntaps * op.seg2.C : 0);      // the GEMM shape tools/layer_times.py reports
     fprintf(stderr, "mitb_conv_phases M %d K %d N %d BN %d nkb %d ctas %d tiles %llu first_wait %llu main %llu wgmma_wait %llu epilogue %llu\n",
             N * op.Ho * op.Wo, K, op.out.C, BN, p.nkb, grid, ph[4], ph[0], ph[1], ph[2], ph[3]);
   }

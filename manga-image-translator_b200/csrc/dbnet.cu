@@ -120,7 +120,7 @@ static void run_block(Exec& e, const CnBlock& b, const View& x, const View& out)
   // Operand fusion along LN -> fc1 -> GELU -> fc2 when both GEMMs run on the TMA-fed kernel: the LayerNorm kernel and fc1's
   // epilogue store the NEXT GEMM's bf16 hi/mid operands into the bytes of `t` / `hid` (same size as the fp32 tensors they
   // replace), so neither GEMM needs a split pass and the normalised / hidden activations never exist in fp32.
-  const bool fuse = conv_tma_capable(op1) && conv_tma_capable(op2) && conv_uses_tma(op1) && conv_uses_tma(op2);
+  const bool fuse = conv_uses_tma(op1) && conv_uses_tma(op2);
   SplitView ts, hs;
   if (fuse) { ts = Exec::alias_split(t); hs = Exec::alias_split(hid); op1.in_sv = ts; op1.out_sv = hs; op1.out.p = nullptr; op2.in_sv = hs; }
   if (b.dense) {
@@ -153,7 +153,7 @@ static void run_stage(Exec& e, const CnStage& s, const View& x, const View& out)
     ConvOp op = Exec::op_from(s.ds, t, d, 2);
     // LayerNorm2d -> 2x2 stride-2 conv: the LN kernel writes the conv's bf16 hi/mid operands directly (no split pass)
     SplitView ts;
-    if (conv_tma_capable(op) && conv_uses_tma(op)) { ts = Exec::alias_split(t); op.in_sv = ts; }
+    if (conv_uses_tma(op)) { ts = Exec::alias_split(t); op.in_sv = ts; }
     e.layernorm(x, t, s.ds_ln_w, s.ds_ln_b, kLnEps, nullptr, nullptr, 1, ts.valid() ? &ts : nullptr);
     e.conv(op);
     cur = d;

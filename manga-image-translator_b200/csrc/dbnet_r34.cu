@@ -122,8 +122,6 @@ DbnetR34Model* dbnet_r34_build(Ctx& ctx, const Weights& W) {
 
 void dbnet_r34_free(DbnetR34Model* m) { delete m; }
 
-static bool on_tma(const ConvOp& op) { return conv_tma_capable(op) && conv_uses_tma(op); }
-
 // ResNet34 layers 1-4 after the max pool.  Operand fusion where every conv involved runs on the TMA-fed kernel: the max pool and
 // each block's conv2 epilogue also store the NEXT block's input as bf16 hi/mid operands (read by its conv1 and downsample), and
 // conv1's epilogue stores only conv2's operands; otherwise the fp32 tensors are written and the convs split them themselves.  The
@@ -152,7 +150,7 @@ static void run_backbone(Exec& e, const DbnetR34Model& m, const View& s0, const 
       s.c2 = Exec::op_from(b.c2, t, y); s.c2.act = ACT_RELU;
       if (b.has_ds) { View d = ws.view(n, Ho, Wo, C); s.ds = Exec::op_from(b.ds, x, d, b.stride); s.c2.add0 = d; }
       else s.c2.add0 = x;
-      s.c1_tma = on_tma(s.c1); s.c2_tma = on_tma(s.c2); s.ds_tma = b.has_ds && on_tma(s.ds);     // decided on the unfused ops
+      s.c1_tma = conv_uses_tma(s.c1); s.c2_tma = conv_uses_tma(s.c2); s.ds_tma = b.has_ds && conv_uses_tma(s.ds);     // decided on the unfused ops
       if (s.c1_tma && s.c2_tma) { s.c1.out_sv = ts; s.c1.out.p = nullptr; s.c2.in_sv = ts; }
       steps.push_back(s);
       x = y; xs_prev = xs;

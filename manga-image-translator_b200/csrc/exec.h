@@ -11,13 +11,23 @@ struct Exec {
   static ConvOp op_from(const ConvW& w, const View& in, const View& out, int stride = 1, int pad_mode = PAD_ZERO) {
     MITB_CHECK(in.C == w.Cin, "conv: input has %d channels, weight expects %d", in.C, w.Cin);
     MITB_CHECK(out.C == w.Cout, "conv: output has %d channels, weight produces %d", out.C, w.Cout);
-    ConvOp op; op.in = in; op.out = out; op.w = w.w; op.ldw = w.ldw; op.ntaps = w.ntaps;
-    for (int t = 0; t < w.ntaps; ++t) { op.tdy[t] = w.tdy[t]; op.tdx[t] = w.tdx[t]; }
+    ConvOp op; op.in = in; op.out = out; op.wt = w;
     op.sy = op.sx = stride; op.pad = pad_mode; op.Ho = out.H; op.Wo = out.W;
     op.scale = w.scale; op.shift = w.shift;
-    op.wh = w.wh; op.wm = w.wm; op.tc_bn = w.tc_bn; op.tc_kpad = w.tc_kpad; op.tc_npad = w.tc_npad; op.tmh = w.tmh; op.tmm = w.tmm;
-    op.whp = w.whp; op.wmp = w.wmp; op.tc_cp = w.tc_cp;
-    op.w8h = w.w8h; op.w8m = w.w8m; op.w8_kh = w.w8_kh; op.w8_kw = w.w8_kw;
+    return op;
+  }
+  // Two K segments accumulated by one launch (FFC: conv1x1(U) + conv3x3_{l->g}(x_l)): segment 1 is `a` over `in`, segment 2 is `b`
+  // over a pre-split tensor the caller sets in seg2 (sv, coff, pad), and ab = Loader::cat_k(a, b) holds the tensor-core weights of
+  // both.  The epilogue's scale / shift are a's.
+  static ConvOp op_from2(const ConvW& a, const ConvW& b, const ConvW& ab, const View& in, const View& out, int stride = 1,
+                         int pad_mode = PAD_ZERO) {
+    MITB_CHECK(ab.Cout == a.Cout && ab.Cin == a.ntaps * a.Cin + b.ntaps * b.Cin, "conv: merged weight does not hold both K segments");
+    ConvOp op = op_from(a, in, out, stride, pad_mode);
+    op.wt = ab;                          // K rows a's then b's: segment 1 keeps a's channels and taps
+    op.wt.Cin = a.Cin; op.wt.ntaps = a.ntaps;
+    for (int t = 0; t < a.ntaps; ++t) { op.wt.tdy[t] = a.tdy[t]; op.wt.tdx[t] = a.tdx[t]; }
+    op.seg2.C = b.Cin; op.seg2.ntaps = b.ntaps;
+    for (int t = 0; t < b.ntaps; ++t) { op.seg2.tdy[t] = b.tdy[t]; op.seg2.tdx[t] = b.tdx[t]; }
     return op;
   }
   void conv(const ConvOp& op) { if (!dry) launch_conv(op, st); }

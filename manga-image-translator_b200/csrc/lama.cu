@@ -148,11 +148,9 @@ static FfcFastOps ffc_fast_ops(const FfcLayer& l, const SplitView& Xs, const Spl
   o.fu = Exec::op_from(l.fu, shape_view(n, h, w2, 384), FP); o.fu.in_sv = SPs; o.fu.act = ACT_RELU;
   {
     View yg = Yf ? Yf->slice(128, 384) : shape_view(n, h, w, 384);
-    ConvOp op = Exec::op_from(l.sp2, shape_view(n, h, w, 192), yg);
-    op.wh = l.sp2m.wh; op.wm = l.sp2m.wm; op.tc_bn = l.sp2m.tc_bn; op.tc_kpad = l.sp2m.tc_kpad; op.tc_npad = l.sp2m.tc_npad;
+    ConvOp op = Exec::op_from2(l.sp2, l.l2g, l.sp2m, shape_view(n, h, w, 192), yg);
     op.in_sv = Us;
-    op.seg2.sv = Xs; op.seg2.coff = 0; op.seg2.C = 128; op.seg2.ntaps = l.l2g.ntaps; op.seg2.pad = PAD_REFLECT;
-    for (int t = 0; t < l.l2g.ntaps; ++t) { op.seg2.tdy[t] = l.l2g.tdy[t]; op.seg2.tdx[t] = l.l2g.tdx[t]; }
+    op.seg2.sv = Xs; op.seg2.coff = 0; op.seg2.pad = PAD_REFLECT;
     op.act = ACT_RELU;
     if (res) op.add1 = res->slice(128, 384);
     op.out_sv = Ys; op.out_sv_coff = 128;

@@ -2,6 +2,7 @@
 // Layout convention: activations are NHWC fp32 "views" (a channel slice of a wider tensor), so channel
 // concatenation (DBNet skip connections, LaMa local|global halves) never costs a copy.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -74,16 +75,27 @@ enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_SILU = 3, ACT_SIGMOID =
 enum Pad { PAD_ZERO = 0, PAD_REFLECT = 1 };
 constexpr int kMaxTaps = 49;
 
-struct alignas(64) TmaDesc { uint64_t q[16]; };   // opaque CUtensorMap (128 bytes)
+// conv weight handle produced at load time
+struct ConvW {
+  const float* w = nullptr;           // [ntaps*Cin][ldw] K-major rows, ldw = round4(Cout)
+  int ldw = 0, Cin = 0, Cout = 0, ntaps = 1;
+  int8_t tdy[kMaxTaps] = {0}, tdx[kMaxTaps] = {0};   // input offset of each tap relative to (oy*sy, ox*sx)
+  const float* scale = nullptr; const float* shift = nullptr;   // folded BN / bias (may be null)
+  // tensor-core copies of the weights (conv_tc.cu): bf16 hi/mid [tc_npad][tc_kpad], K-major; null -> SIMT path only
+  const uint16_t* wh = nullptr; const uint16_t* wm = nullptr; int tc_bn = 0, tc_kpad = 0, tc_npad = 0;
+  // per-tap channel-padded copies [tc_npad][ntaps*tc_cp] for the TMA-fed kernel when Cin % 64 != 0 (null otherwise)
+  const uint16_t* whp = nullptr; const uint16_t* wmp = nullptr; int tc_cp = 0;
+  // Cin = 4 stems on the tensor cores: weights packed [tc_npad][kh*64], k = ky*64 + kx*8 + c (kx < kw <= 8, c < 4, rest zero): one
+  // K block per kernel row, fed by an OVERLAPPING-stride tensor map over the 8-channel-padded input (conv_tma.cu)
+  const uint16_t* w8h = nullptr; const uint16_t* w8m = nullptr; int w8_kh = 0, w8_kw = 0;
+};
 
 // Alignment: the base pointers of in / out / add0 / add1 (and of every split tensor) must be 16-byte aligned, in_scale / in_shift
 // too: the SIMT kernel reads and writes float4 whenever cs and coff are multiples of 4 and the split kernels move 16-byte packs.
 // scale / shift / mul1 / os_scale / os_shift need 4 bytes (the tensor-core epilogue reads them as float2 only when 8-byte aligned).
 struct ConvOp {
   View in, out;                       // out grid may be larger than the logical (Ho,Wo) grid (transposed phases)
-  const float* w = nullptr;           // [ntaps*Cin][ldw] K-major rows, ldw = round4(Cout)
-  int ldw = 0, ntaps = 1;
-  int8_t tdy[kMaxTaps] = {0}, tdx[kMaxTaps] = {0};   // input offset of each tap relative to (oy*sy, ox*sx)
+  ConvW wt;                           // weights and taps; the epilogue reads scale / shift below, not wt's
   int sy = 1, sx = 1, pad = PAD_ZERO;
   int Ho = 0, Wo = 0;                 // logical output grid of this launch
   int oy_mul = 1, oy_add = 0, ox_mul = 1, ox_add = 0;   // out pixel = (oy*oy_mul+oy_add, ox*ox_mul+ox_add)
@@ -98,16 +110,8 @@ struct ConvOp {
   // Output-sparsity hint for the TMA conv kernel: uint8 [N][Ho][Wo] over this launch's LOGICAL output grid; output tiles without a
   // non-zero entry are skipped (left unwritten).  The caller guarantees that nothing it still needs depends on skipped pixels.
   const uint8_t* need_px = nullptr;
-  const float* scale = nullptr; const float* shift = nullptr; const float* mul1 = nullptr;
+  const float* scale = nullptr; const float* shift = nullptr; const float* mul1 = nullptr;   // initialised from wt, callers override
   int act = ACT_NONE;
-  // tensor-core copies of the weights (conv_tc.cu): bf16 hi/mid [tc_npad][tc_kpad], K-major; null -> SIMT path only
-  const uint16_t* wh = nullptr; const uint16_t* wm = nullptr; int tc_bn = 0, tc_kpad = 0, tc_npad = 0;
-  TmaDesc tmh, tmm;                   // TMA descriptors of wh / wm
-  // per-tap channel-padded copies [tc_npad][ntaps*tc_cp] for the TMA-fed kernel when Cin % 64 != 0 (null otherwise)
-  const uint16_t* whp = nullptr; const uint16_t* wmp = nullptr; int tc_cp = 0;
-  // Cin = 4 stems on the tensor cores: weights packed [tc_npad][kh*64], k = ky*64 + kx*8 + c (kx < kw <= 8, c < 4, rest zero): one
-  // K block per kernel row, fed by an OVERLAPPING-stride tensor map over the 8-channel-padded input (conv_tma.cu)
-  const uint16_t* w8h = nullptr; const uint16_t* w8m = nullptr; int w8_kh = 0, w8_kw = 0;
   // TMA-path operand fusion (only legal when conv_uses_tma() holds for the op):
   //  * in_sv valid  -> the input already exists as bf16 hi/mid (written by its producer); channels [in_sv_coff, +in.C) of it are
   //                    this conv's input, `in` then only carries the shape; the split pass is skipped;
@@ -118,15 +122,38 @@ struct ConvOp {
   SplitView out_sv; int out_sv_coff = 0;
   const float* os_scale = nullptr; const float* os_shift = nullptr; int os_relu = 0;
   // optional second K segment accumulated into the same output (FFC: conv1x1(U) + conv3x3_{l->g}(x_l)): pre-split input only.
-  // The weight rows of segment 2 follow those of segment 1 in wh/wm (K-major, both Cin multiples of 64).
+  // The weight rows of segment 2 follow those of segment 1 in wt.wh / wt.wm (K-major, both Cin multiples of 64; Exec::op_from2).
   struct Seg2 { SplitView sv; int coff = 0, C = 0, ntaps = 0, pad = PAD_ZERO; int8_t tdy[kMaxTaps] = {0}, tdx[kMaxTaps] = {0}; } seg2;
   // optional fused row statistics (vocabulary head): no tensor output, per (row, column-block) partials
   float* stat_max = nullptr; float* stat_sum = nullptr; int* stat_idx = nullptr; int stat_ld = 0;
 };
 
-void launch_conv(const ConvOp& op, cudaStream_t st);
-// Host-side record of what launch_conv() ran (test hook mitb_test_conv): null by default, and nothing is recorded then.
+// conv.cu: which kernel runs an op.  conv_plan() is the only place that decides it; launch_conv() validates the op, runs the
+// planned kernel under the plan's profiler class, and the predicates below are derived from the plan.
 enum ConvKernel { CK_SIMT = 1, CK_FEWOUT, CK_THIN, CK_GATHER, CK_GATHER_SPLITK, CK_TMA, CK_STEM8 };
+struct ConvPlan {
+  ConvKernel kernel = CK_SIMT;
+  int splits = 1;                     // split-K factor of the gather kernel
+  const char* prof = "conv_simt";     // profiler class
+  bool sparse = false;                // output-sparse launch: the executed work depends on device data, no flop / byte claim
+};
+ConvPlan conv_plan(const ConvOp& op);
+void launch_conv(const ConvOp& op, cudaStream_t st);
+bool conv_uses_tma(const ConvOp& op);      // true when launch_conv() will run this op on the TMA-fed tensor-core kernel
+bool conv_tma_capable(const ConvOp& op);   // the op CAN run there (launch_conv() does so whenever in_sv / out_sv / seg2 is set)
+int conv_stat_blocks(const ConvOp& op);    // number of column blocks the row-stat epilogue writes per row
+// the kernels' entry points: *_supported() says whether the kernel can run the op, launch_conv_*() runs it as planned
+bool conv_thin_supported(const ConvOp& op);                         // conv_thin.cu
+void launch_conv_thin(const ConvOp& op, cudaStream_t st);
+void launch_conv_simt(const ConvOp& op, bool fewout, cudaStream_t st);   // conv_simt.cu
+bool conv_tc_supported(const ConvOp& op);                           // conv_tc.cu: register-gather wgmma kernel
+void launch_conv_tc(const ConvOp& op, int splits, cudaStream_t st);
+bool conv_tma_supported(const ConvOp& op);                          // conv_tma.cu: TMA-fed wgmma kernel
+bool conv_stem8_supported(const ConvOp& op);
+void launch_conv_tma(const ConvOp& op, bool stem, cudaStream_t st);   // stem: a refused stem map disables stem8, runs launch_conv() again
+// weight tensor map (conv_tma.cu): bf16 [rows][kdim] K-major, box {64 k, bn}, 128-byte swizzle; rows beyond `rows` are zero filled
+void make_w_tmap(CUtensorMap* m, const uint16_t* base, int kdim, int rows, int bn);
+// Host-side record of what launch_conv() ran (test hook mitb_test_conv): null by default, and nothing is recorded then.
 struct ConvTrace { int kernel = 0, bn = 0, splits = 1, vec2 = -1, tma_act = -2, split_reused = 0, convs = 0, staged = -1; };
 extern ConvTrace* g_conv_trace;
 inline void conv_trace(int kernel, int bn, int splits, int vec2, int tma_act, bool reused, int staged = -1) {
@@ -140,13 +167,10 @@ bool conv_tma_bn_candidate(int Cout, int bn);
 bool conv_tc_enabled();
 bool conv_tma_enabled();
 void conv_tma_set_enabled(bool on);
-bool conv_uses_tma(const ConvOp& op);      // true when launch_conv() will run this op on the TMA-fed tensor-core kernel
-bool conv_tma_capable(const ConvOp& op);   // the op CAN run there (launch_conv() does so whenever in_sv / out_sv / seg2 is set)
 // fill the reflect halo of channels [coff, coff+C) of a split tensor from its interior (pad <= 3)
 void launch_split_halo(const SplitView& sv, int coff, int C, cudaStream_t st);
 // fp32 NHWC view -> split tensor (channels [coff, coff+in.C)), optional BN+ReLU prologue, halo by reflection
 void launch_split(const View& in, const SplitView& sv, int coff, const float* in_scale, const float* in_shift, int in_relu, cudaStream_t st);
-int conv_stat_blocks(const ConvOp& op);   // number of column blocks the row-stat epilogue writes per row
 void launch_rowstat_final(const float* pmax, const float* psum, const int* pidx, int rows, int nblk,
                           int* idx, float* logprob, cudaStream_t st);
 
@@ -231,17 +255,6 @@ struct DevBlob {                       // owning device allocation for repacked 
   ~DevBlob() { free_all(); }
 };
 
-// conv weight handle produced at load time
-struct ConvW {
-  const float* w = nullptr; int ldw = 0, Cin = 0, Cout = 0, ntaps = 1;
-  int8_t tdy[kMaxTaps] = {0}, tdx[kMaxTaps] = {0};
-  const float* scale = nullptr; const float* shift = nullptr;   // folded BN / bias (may be null)
-  const uint16_t* wh = nullptr; const uint16_t* wm = nullptr; int tc_bn = 0, tc_kpad = 0, tc_npad = 0;
-  TmaDesc tmh, tmm;
-  const uint16_t* whp = nullptr; const uint16_t* wmp = nullptr; int tc_cp = 0;   // per-tap channel-padded copies (conv_tma.cu)
-  const uint16_t* w8h = nullptr; const uint16_t* w8m = nullptr; int w8_kh = 0, w8_kw = 0;   // Cin = 4 stem packing (conv_tma.cu)
-};
-struct DevBlob;
 void conv_tc_prepare(ConvW& cw, DevBlob& blob, cudaStream_t st);   // build the bf16 hi/mid tensor-core weight copies
 void conv_tc_set_enabled(bool on);
 
@@ -359,6 +372,25 @@ inline int device_sm_count() {
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 __device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+
+// the conv epilogue's activation (enum Act)
+__device__ __forceinline__ float apply_act(float v, int act) {
+  switch (act) {
+    case ACT_RELU: return fmaxf(v, 0.f);
+    case ACT_GELU: return 0.5f * v * (1.f + erff(v * 0.70710678118654752440f));
+    case ACT_SILU: return v / (1.f + expf(-v));
+    case ACT_SIGMOID: return 1.f / (1.f + expf(-v));
+    case ACT_SIGMOID2: { float s = 1.f / (1.f + expf(-v)); return 1.f / (1.f + expf(-s)); }
+    case ACT_CLAMP01: return fminf(fmaxf(v, 0.f), 1.f);
+    default: return v;
+  }
+}
+// reflect padding (PyTorch 'reflect', no edge repeat) of index i into [0, n), for |i| reaching at most n - 1 past an edge
+__device__ __forceinline__ int reflect_idx(int i, int n) {
+  if (i < 0) i = -i;
+  if (i >= n) i = 2 * n - 2 - i;
+  return i;
+}
 
 extern unsigned long g_launch_epoch;     // bumped by EVERY kernel launch of the library (conv_tma.cu's split reuse keys on it)
 inline void count_launch() { ++g_launch_epoch; if (g_launch_counter) ++*g_launch_counter; }

@@ -111,8 +111,6 @@ OcrModel* ocr_build(Ctx& ctx, const Weights& W) {
 
 void ocr_free(OcrModel* m) { delete m; }
 
-static bool fusable(const ConvOp& op) { return conv_tma_capable(op) && conv_uses_tma(op); }   // runs on the TMA kernel, no split-K
-
 // BN(+ReLU) prologue of whichever conv consumes a tensor next (pre-activation ResNet: applied by the PRODUCER's epilogue when fused)
 struct NextBn { const float* s = nullptr; const float* b = nullptr; int relu = 0; };
 
@@ -128,14 +126,14 @@ static void run_block(Exec& e, const OcrBlock& b, const View& x, const View& out
   if (xs.valid()) op1.in_sv = xs; else { op1.in_scale = b.bn1_s; op1.in_shift = b.bn1_b; op1.in_relu = 1; }
   View res = x;
   ConvOp op2 = Exec::op_from(b.conv2, y1, out);
-  if (fusable(op1) && fusable(op2)) { SplitView ys = Exec::alias_split(y1); op1.out_sv = ys; op1.out.p = nullptr; op2.in_sv = ys; }
+  if (conv_uses_tma(op1) && conv_uses_tma(op2)) { SplitView ys = Exec::alias_split(y1); op1.out_sv = ys; op1.out.p = nullptr; op2.in_sv = ys; }
   e.conv(op1);
   if (b.has_ds) {
     res = ws.view(x.N, x.H, x.W, b.ds.Cout);
     ConvOp op = Exec::op_from(b.ds, x, res); op.in_scale = b.ds_s; op.in_shift = b.ds_b; op.in_relu = 0; e.conv(op);
   }
   op2.add1 = res;
-  if (outs && outs->valid() && fusable(op2)) { op2.out_sv = *outs; op2.os_scale = nxt.s; op2.os_shift = nxt.b; op2.os_relu = nxt.relu; }
+  if (outs && outs->valid() && conv_uses_tma(op2)) { op2.out_sv = *outs; op2.os_scale = nxt.s; op2.os_shift = nxt.b; op2.os_relu = nxt.relu; }
   else if (outs) *outs = SplitView();
   e.conv(op2);
   ws.release(mk);
@@ -181,11 +179,11 @@ void ocr_run(Ctx& ctx, OcrModel& m, const float* x_nchw, const uint8_t* x_u8, in
       if (l < 3) {
         View t = ws.view(cur.N, cur.H, cur.W, chans[l]);
         ConvOp op = Exec::op_from(m.tail[l].conv, cur, t);
-        if (cur_s.valid() && fusable(op)) op.in_sv = cur_s; else { op.in_scale = m.tail[l].s; op.in_shift = m.tail[l].b; op.in_relu = 1; }
+        if (cur_s.valid() && conv_uses_tma(op)) op.in_sv = cur_s; else { op.in_scale = m.tail[l].s; op.in_shift = m.tail[l].b; op.in_relu = 1; }
         cur_s = SplitView();
         if (l == 2) {                             // conv3 feeds layer4.0.conv1 directly (no pool, no downsample path): emit its operands
           SplitView ts = ws.split_view(cur.N, cur.H, cur.W, chans[l]);
-          if (fusable(op) && !m.layer[3][0].has_ds) { op.out_sv = ts; op.os_scale = m.layer[3][0].bn1_s; op.os_shift = m.layer[3][0].bn1_b; op.os_relu = 1; cur_s = ts; }
+          if (conv_uses_tma(op) && !m.layer[3][0].has_ds) { op.out_sv = ts; op.os_scale = m.layer[3][0].bn1_s; op.os_shift = m.layer[3][0].bn1_b; op.os_relu = 1; cur_s = ts; }
         }
         e.conv(op);
         if (l == 0) { View pl = ws.view(n, 12, w2, chans[l]); e.avgpool(t, pl, 0); cur = pl; }
@@ -197,9 +195,9 @@ void ocr_run(Ctx& ctx, OcrModel& m, const float* x_nchw, const uint8_t* x_u8, in
     View x = ws.view(n, 1, T, 320);               // tokens [n*T, 320]
     {
       ConvOp op41 = Exec::op_from(m.t41.conv, cur, f1); op41.sy = 2; op41.sx = 1;
-      if (cur_s.valid() && fusable(op41)) op41.in_sv = cur_s; else { op41.in_scale = m.t41.s; op41.in_shift = m.t41.b; op41.in_relu = 1; }
+      if (cur_s.valid() && conv_uses_tma(op41)) op41.in_sv = cur_s; else { op41.in_scale = m.t41.s; op41.in_shift = m.t41.b; op41.in_relu = 1; }
       ConvOp op42 = Exec::op_from(m.t42.conv, f1, x);
-      if (fusable(op41) && fusable(op42)) {      // conv4_1's epilogue applies bn4_2 + relu and writes conv4_2's operands
+      if (conv_uses_tma(op41) && conv_uses_tma(op42)) {      // conv4_1's epilogue applies bn4_2 + relu and writes conv4_2's operands
         SplitView fs = Exec::alias_split(f1);
         op41.out_sv = fs; op41.os_scale = m.t42.s; op41.os_shift = m.t42.b; op41.os_relu = 1; op41.out.p = nullptr; op42.in_sv = fs;
       } else { op42.in_scale = m.t42.s; op42.in_shift = m.t42.b; op42.in_relu = 1; }
@@ -220,7 +218,7 @@ void ocr_run(Ctx& ctx, OcrModel& m, const float* x_nchw, const uint8_t* x_u8, in
       {
         ConvOp o1 = Exec::op_from(L.l1, z, hid); o1.act = ACT_GELU;
         ConvOp o2 = Exec::op_from(L.l2, hid, x); o2.add1 = x;
-        if (fusable(o1) && fusable(o2)) { SplitView hs = Exec::alias_split(hid); o1.out_sv = hs; o1.out.p = nullptr; o2.in_sv = hs; }
+        if (conv_uses_tma(o1) && conv_uses_tma(o2)) { SplitView hs = Exec::alias_split(hid); o1.out_sv = hs; o1.out.p = nullptr; o2.in_sv = hs; }
         e.conv(o1);
         e.conv(o2);
       }

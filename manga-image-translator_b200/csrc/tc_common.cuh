@@ -152,23 +152,6 @@ __device__ __forceinline__ void wgmma_kblock_x3(float (&acc)[BN / 2], uint64_t d
   }
 }
 
-__device__ __forceinline__ float apply_act_tc(float v, int act) {
-  switch (act) {
-    case ACT_RELU: return fmaxf(v, 0.f);
-    case ACT_GELU: return 0.5f * v * (1.f + erff(v * 0.70710678118654752440f));
-    case ACT_SILU: return v / (1.f + expf(-v));
-    case ACT_SIGMOID: return 1.f / (1.f + expf(-v));
-    case ACT_SIGMOID2: { float s = 1.f / (1.f + expf(-v)); return 1.f / (1.f + expf(-s)); }
-    case ACT_CLAMP01: return fminf(fmaxf(v, 0.f), 1.f);
-    default: return v;
-  }
-}
-__device__ __forceinline__ int reflect_tc(int i, int n) {
-  if (i < 0) i = -i;
-  if (i >= n) i = 2 * n - 2 - i;
-  return i;
-}
-
 // split 8 fp32 values into bf16 hi / mid packs (16 bytes each): 6 instructions per pair
 // (F2FP pack-convert for hi, shift/mask to get hi back as fp32, two FADD for the remainder, F2FP for mid)
 __device__ __forceinline__ void split8(const float (&v)[8], uint4& hi, uint4& mid) {
@@ -220,7 +203,7 @@ __device__ __forceinline__ float act_t(float v, int act_rt) {
   if (ACT == ACT_RELU) return fmaxf(v, 0.f);
   if (ACT == ACT_GELU) return gelu_fast(v);
   if (ACT == ACT_SILU) return v / (1.f + expf(-v));
-  return apply_act_tc(v, act_rt);               // ACT == -1: rare activations, runtime switch
+  return apply_act(v, act_rt);               // ACT == -1: rare activations, runtime switch
 }
 
 

@@ -104,6 +104,12 @@ int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* d, mitb_test_conv_i
     Loader L{W, blob, st};
     ConvW cw = L.conv_padcin("w", 0, d->C);
     for (int t = 0; t < cw.ntaps; ++t) { cw.tdy[t] = (int8_t)(t / d->kw - d->pad_y); cw.tdx[t] = (int8_t)(t % d->kw - d->pad_x); }
+    ConvW w2, cat;                        // FFC's layout (lama.cu): one tensor-core weight whose K rows are segment 1's followed by segment 2's
+    if (d->seg2.hi) {
+      w2 = L.conv_padcin("w2", 0, d->seg2_cin);
+      for (int t = 0; t < w2.ntaps; ++t) { w2.tdy[t] = (int8_t)(t / d->seg2_kw - d->seg2_pad); w2.tdx[t] = (int8_t)(t % d->seg2_kw - d->seg2_pad); }
+      cat = L.cat_k(cw, w2);
+    }
 
     View in; in.p = const_cast<float*>(d->x); in.N = d->N; in.H = d->H; in.W = d->W; in.C = d->C;
     in.cs = d->x ? d->cs : d->C; in.coff = d->x ? d->coff : 0; in.planar = d->planar != 0;
@@ -112,7 +118,8 @@ int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* d, mitb_test_conv_i
     out.cs = d->out ? d->out_cs : d->cout; out.coff = d->out ? d->out_coff : 0; out.planar = d->out_planar != 0;
     MITB_CHECK(!d->out || (d->out_cs > 0 && d->out_coff >= 0 && d->out_coff + d->cout <= d->out_cs), "test_conv: output slice outside cs");
 
-    ConvOp op = Exec::op_from(cw, in, out, d->stride, d->pad_mode == 1 ? PAD_REFLECT : PAD_ZERO);
+    const int pad_mode = d->pad_mode == 1 ? PAD_REFLECT : PAD_ZERO;
+    ConvOp op = d->seg2.hi ? Exec::op_from2(cw, w2, cat, in, out, d->stride, pad_mode) : Exec::op_from(cw, in, out, d->stride, pad_mode);
     op.Ho = Ho; op.Wo = Wo; op.oy_mul = oy_mul; op.oy_add = d->oy_add; op.ox_mul = ox_mul; op.ox_add = d->ox_add;
     op.in_scale = d->in_scale; op.in_shift = d->in_shift; op.in_relu = d->in_relu;
     MITB_CHECK(!op.in_scale == !op.in_shift, "test_conv: in_scale and in_shift go together");
@@ -127,14 +134,7 @@ int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* d, mitb_test_conv_i
     }
     if (d->in_sv.hi) { op.in_sv = split(d->in_sv, d->N, d->H, d->W, d->C); op.in_sv_coff = d->in_sv.coff; }
     if (d->seg2.hi) {
-      // FFC's layout (lama.cu): one tensor-core weight whose K rows are segment 1's followed by segment 2's
-      ConvW w2 = L.conv_padcin("w2", 0, d->seg2_cin);
-      for (int t = 0; t < w2.ntaps; ++t) { w2.tdy[t] = (int8_t)(t / d->seg2_kw - d->seg2_pad); w2.tdx[t] = (int8_t)(t % d->seg2_kw - d->seg2_pad); }
-      const ConvW m = L.cat_k(cw, w2);
-      op.wh = m.wh; op.wm = m.wm; op.tc_bn = m.tc_bn; op.tc_kpad = m.tc_kpad; op.tc_npad = m.tc_npad;
-      op.seg2.sv = split(d->seg2, d->N, Ho, Wo, d->seg2_cin); op.seg2.coff = d->seg2.coff; op.seg2.C = d->seg2_cin;
-      op.seg2.ntaps = w2.ntaps; op.seg2.pad = d->seg2_pad_mode == 1 ? PAD_REFLECT : PAD_ZERO;
-      for (int t = 0; t < w2.ntaps; ++t) { op.seg2.tdy[t] = w2.tdy[t]; op.seg2.tdx[t] = w2.tdx[t]; }
+      op.seg2.sv = split(d->seg2, d->N, Ho, Wo, d->seg2_cin); op.seg2.coff = d->seg2.coff; op.seg2.pad = d->seg2_pad_mode == 1 ? PAD_REFLECT : PAD_ZERO;
     }
     // a fused op on any other kernel would dereference the shape-only views
     MITB_CHECK(!fused || conv_tma_capable(op), "test_conv: this op cannot run on the TMA-fed kernel");
