@@ -275,12 +275,33 @@ typedef struct {             /* what the last conv launch of the call ran */
   int32_t split_reused;      /* @20 launches of this call whose operand split came from the reuse cache */
   int32_t convs;             /* @24 conv launches in this call */
   int32_t staged;            /* @28 conv_tma_kernel: channels per thread of the staged epilogue (4 or 2), 0 register epilogue; -1 other kernels */
-} mitb_test_conv_info;       /* 32 bytes */
+  int32_t epi_sig;           /* @32 staged epilogue: signature that ran (MITB_EPI_* bits, MITB_EPI_GENERIC); -1 other epilogues */
+} mitb_test_conv_info;       /* 36 bytes */
 
 /* Runs the conv `runs` times on `stream`, synchronises, fills *info.  Error (non-zero) for a bad descriptor, a misaligned
  * pointer, a path that cannot take the op, or a force_bn the TMA kernel's N tile choice would never make for this cout. */
 int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* desc, mitb_test_conv_info* info, void* stream);
 int mitb_test_struct_sizes(int* desc_bytes, int* info_bytes);
+
+/* Epilogue signatures of the TMA conv kernel's staged epilogue: which parts of the fused chain a launch has.  A staged launch whose
+ * (activation, signature) pair has a kernel of its own runs it; any other runs MITB_EPI_GENERIC, which tests every part at run time. */
+#define MITB_EPI_ADD0 1
+#define MITB_EPI_SCALE 2
+#define MITB_EPI_SHIFT 4
+#define MITB_EPI_MUL1 8
+#define MITB_EPI_ADD1 16
+#define MITB_EPI_OUT 32
+#define MITB_EPI_OS 64             /* split output out_sv */
+#define MITB_EPI_OS_AFFINE 128     /* os_scale / os_shift */
+#define MITB_EPI_OS_RELU 256
+#define MITB_EPI_GENERIC 512
+/* on = 0 runs every staged launch on the generic signature (as MITB_EPI_GENERIC=1 does), 1 on its own where one exists.
+ * Process-wide; returns the previous setting. */
+int mitb_set_epi_specialise(int on);
+/* The signature a staged launch with activation `act` (enum Act) and chain parts `sig` runs with under the current setting. */
+int mitb_test_epi_signature(int act, int sig);
+/* The (activation, signature) pairs with a kernel of their own: fills up to cap entries, returns how many there are. */
+int mitb_test_epi_signatures(int* act, int* sig, int cap);
 
 #ifdef __cplusplus
 }

@@ -60,9 +60,11 @@ struct TmaParams {
 
 // Phase timing (build with EXTRA=-DMITB_CONV_PHASES, read by tools/conv_phases.py): clock64 sums over all consumer warpgroups
 // of a launch for [0] the wait on a tile's first full barrier, [1] the main loop, [2] wgmma_wait<0>, [3] the epilogue; [4] counts
-// processed tiles.  The default build contains none of it.
+// processed tiles; [5..7] split a staged epilogue into chunk writes + barriers, column vector loads and the row walk (sums over
+// all consumer threads).  The default build contains none of it.
+constexpr int N_PHASES = 8;
 #ifdef MITB_CONV_PHASES
-__device__ unsigned long long g_conv_phases[5];
+__device__ unsigned long long g_conv_phases[N_PHASES];
 #define PHASE_CLOCK(v) v = clock64()
 #else
 #define PHASE_CLOCK(v)
@@ -110,15 +112,39 @@ template <int W> __device__ __forceinline__ void st_bf16_w(uint16_t* q, const ui
 template <> __device__ __forceinline__ void st_bf16_w<4>(uint16_t* q, const uint32_t (&v)[2]) { *reinterpret_cast<uint2*>(q) = make_uint2(v[0], v[1]); }
 template <> __device__ __forceinline__ void st_bf16_w<2>(uint16_t* q, const uint32_t (&v)[1]) { *reinterpret_cast<uint32_t*>(q) = v[0]; }
 
+// Rows in flight per thread in epilogue_staged: as many as the registers left next to the accumulators hold without spills
+// (ptxas -v over every instantiation).  Each row in flight holds W chunk values, W per residual operand and two pixel indices.  The
+// generic signature keeps registers for every operand: at BN = 128 the 96 accumulator registers still live during the first chunk
+// leave room for one 16-byte row only.
+template <int SIG, int BN, int W> __host__ __device__ constexpr int epi_rows() {
+  if (SIG == EPI_GENERIC) return (BN == 128 ? 4 : 8) / W;
+  const int res = ((SIG & EPI_ADD0) ? 1 : 0) + ((SIG & EPI_ADD1) ? 1 : 0);
+  return res == 0 ? 32 / W : res == 1 ? 16 / W : (BN == 128 ? 4 : 8) / W;
+}
+
+#ifdef MITB_CONV_PHASES
+#define EPI_CLOCK(i) do { const long long now_ = clock64(); ep[i] += now_ - ep_t; ep_t = now_; } while (0)
+#else
+#define EPI_CLOCK(i)
+#endif
+
 // The fused chain of one 128 x BN tile: acc0 holds rows 0-63, acc1 rows 64-127 (fragment layout of epilogue_tile; `row` is this
 // thread's first row); both are consumed.  rowpix(r, ...) as in epilogue_tile; rowm(r) is the tile row's index in the logical output
 // grid, which is the pixel index of out / add0 / add1 whenever there is a split output (launch_conv_tma admits out_sv only on the conv's
-// own grid), so the row table needs one entry per row.  `bar` is this warpgroup's named barrier.
-template <int ACT, int BN, int W, class RowPix, class RowM>
+// own grid), so the row table needs one entry per row.  `bar` is this warpgroup's named barrier.  SIG (EpiSig) is the launch's
+// epilogue signature: only its operands are declared, loaded and applied.  ep: phase-timer sums (chunk writes + barriers, column
+// vector loads, row walk), MITB_CONV_PHASES builds only.
+template <int ACT, int BN, int W, int SIG, class RowPix, class RowM>
 __device__ __forceinline__ void epilogue_staged(const EpiParams& e, float (&acc0)[BN / 2], float (&acc1)[BN / 2], int row, int n0, float* chunk,
-                                                int* rtab, int bar, RowPix rowpix, RowM rowm) {
-  constexpr int TPR = EPI_CW / W, RPP = TC_BM / TPR, NR = (BN == 128 ? 4 : 8) / W;   // threads per row, rows per pass, rows in flight
-  // (at BN = 128 the 96 accumulator registers still live during the first chunk leave room for one 16-byte row only: 2 spill)
+                                                int* rtab, int bar, RowPix rowpix, RowM rowm, long long* ep) {
+  constexpr int TPR = EPI_CW / W, RPP = TC_BM / TPR, NR = epi_rows<SIG, BN, W>();   // threads per row, rows per pass, rows in flight
+  static_assert((TC_BM / RPP) % NR == 0, "rows in flight must divide a thread's rows");
+  const bool add0 = epi_has<SIG, EPI_ADD0>(e.add0), add1 = epi_has<SIG, EPI_ADD1>(e.add1), out = epi_has<SIG, EPI_OUT>(e.out);
+  const bool os = epi_has<SIG, EPI_OS>(e.os_hi), os_aff = epi_has<SIG, EPI_OS_AFFINE>(e.os_scale);
+  constexpr bool kA0 = SIG == EPI_GENERIC || (SIG & EPI_ADD0), kA1 = SIG == EPI_GENERIC || (SIG & EPI_ADD1);   // arrays to declare
+#ifdef MITB_CONV_PHASES
+  long long ep_t = clock64();
+#endif
   const int t = threadIdx.x & 127, cl = 2 * (t & 3);
   const int q = t % TPR, r0 = t / TPR;
   named_bar_sync(bar, 128);                           // the previous tile's reads of the chunk and the row table are done
@@ -126,8 +152,8 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& e, float (&acc0
     // row table: pixel index of the split output if there is one, else of out; -1 outside the output
     int nimg = 0, oy = 0, ox = 0;
     const bool ok = rowpix(t, nimg, oy, ox);
-    rtab[t] = !ok ? -1 : e.os_hi ? (nimg * e.os_Hp + oy + e.os_pt) * e.os_Wp + ox + e.os_pl
-                                 : (nimg * e.oH + oy * e.oy_mul + e.oy_add) * e.oW + ox * e.ox_mul + e.ox_add;
+    rtab[t] = !ok ? -1 : os ? (nimg * e.os_Hp + oy + e.os_pt) * e.os_Wp + ox + e.os_pl
+                            : (nimg * e.oH + oy * e.oy_mul + e.oy_add) * e.oW + ox * e.ox_mul + e.ox_add;
   }
 #pragma unroll 1
   for (int c0 = n0; c0 < n0 + BN && c0 < e.Cout; c0 += EPI_CW) {
@@ -146,47 +172,54 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& e, float (&acc0
       }
     }
     named_bar_sync(bar, 128);
+    EPI_CLOCK(0);
     const int c = c0 + W * q;                           // Cout is a multiple of W: a thread's channels are all inside or all past it
     if (c < e.Cout) {
-      float sc[W], sh[W], m1[W], os[W], ot[W];
+      float sc[W], sh[W], m1[W], os_s[W], os_t[W];
 #pragma unroll
-      for (int k = 0; k < W; ++k) sc[k] = sh[k] = m1[k] = os[k] = ot[k] = 0.f;
-      if (e.scale) ldg_w<W>(sc, e.scale + c);
-      if (e.shift) ldg_w<W>(sh, e.shift + c);
-      if (e.mul1) ldg_w<W>(m1, e.mul1 + c);
-      if (e.os_scale) { ldg_w<W>(os, e.os_scale + c); ldg_w<W>(ot, e.os_shift + c); }
+      for (int k = 0; k < W; ++k) sc[k] = sh[k] = m1[k] = os_s[k] = os_t[k] = 0.f;
+      if (epi_has<SIG, EPI_SCALE>(e.scale)) ldg_w<W>(sc, e.scale + c);
+      if (epi_has<SIG, EPI_SHIFT>(e.shift)) ldg_w<W>(sh, e.shift + c);
+      if (epi_has<SIG, EPI_MUL1>(e.mul1)) ldg_w<W>(m1, e.mul1 + c);
+      if (os_aff) { ldg_w<W>(os_s, e.os_scale + c); ldg_w<W>(os_t, e.os_shift + c); }
+      EPI_CLOCK(1);
 #pragma unroll 1
       for (int i0 = 0; i0 < TC_BM / RPP; i0 += NR) {
-        // the residual loads of all rows in flight ahead of the first store: add0 / add1 may alias out
+        // the chunk reads and residual loads of all rows in flight ahead of the first chain and store: add0 / add1 may alias out
         int px[NR], opx[NR];
-        float a0[NR][W], a1[NR][W];
+        float v[NR][W], a0[kA0 ? NR : 1][W], a1[kA1 ? NR : 1][W];
 #pragma unroll
         for (int i = 0; i < NR; ++i) {
           const int r = r0 + (i0 + i) * RPP;
           px[i] = rtab[r];
-          opx[i] = e.os_hi ? rowm(r) : px[i];
+          opx[i] = os ? rowm(r) : px[i];
+          ld_w<W>(v[i], chunk + chunk_off(r, W * q));
+          if constexpr (kA0) {
 #pragma unroll
-          for (int k = 0; k < W; ++k) a0[i][k] = a1[i][k] = 0.f;
-          if (px[i] >= 0) {
-            if (e.add0) ld_w<W>(a0[i], e.add0 + (size_t)opx[i] * e.add0_cs + e.add0_coff + c);
-            if (e.add1) ld_w<W>(a1[i], e.add1 + (size_t)opx[i] * e.add1_cs + e.add1_coff + c);
+            for (int k = 0; k < W; ++k) a0[i][k] = 0.f;
+            if (add0 && px[i] >= 0) ld_w<W>(a0[i], e.add0 + (size_t)opx[i] * e.add0_cs + e.add0_coff + c);
+          }
+          if constexpr (kA1) {
+#pragma unroll
+            for (int k = 0; k < W; ++k) a1[i][k] = 0.f;
+            if (add1 && px[i] >= 0) ld_w<W>(a1[i], e.add1 + (size_t)opx[i] * e.add1_cs + e.add1_coff + c);
           }
         }
 #pragma unroll
         for (int i = 0; i < NR; ++i) {
           if (px[i] < 0) continue;
-          float v[W];
-          ld_w<W>(v, chunk + chunk_off(r0 + (i0 + i) * RPP, W * q));
+          const int ia0 = kA0 ? i : 0, ia1 = kA1 ? i : 0;
 #pragma unroll
           for (int k = 0; k < W; k += 2)
-            epi_chain2<ACT>(e, v[k], v[k + 1], make_float2(a0[i][k], a0[i][k + 1]), make_float2(sc[k], sc[k + 1]), make_float2(sh[k], sh[k + 1]),
-                            make_float2(m1[k], m1[k + 1]), make_float2(a1[i][k], a1[i][k + 1]));
-          if (e.out) st_w<W>(e.out + (size_t)opx[i] * e.out_cs + e.out_coff + c, v);
-          if (e.os_hi) {
+            epi_chain2<ACT, SIG>(e, v[i][k], v[i][k + 1], kA0 ? make_float2(a0[ia0][k], a0[ia0][k + 1]) : make_float2(0.f, 0.f),
+                                 make_float2(sc[k], sc[k + 1]), make_float2(sh[k], sh[k + 1]), make_float2(m1[k], m1[k + 1]),
+                                 kA1 ? make_float2(a1[ia1][k], a1[ia1][k + 1]) : make_float2(0.f, 0.f));
+          if (out) st_w<W>(e.out + (size_t)opx[i] * e.out_cs + e.out_coff + c, v[i]);
+          if (os) {
             uint32_t hh[W / 2], mm[W / 2];
 #pragma unroll
             for (int k = 0; k < W; k += 2)
-              epi_split2(e, v[k], v[k + 1], make_float2(os[k], os[k + 1]), make_float2(ot[k], ot[k + 1]), hh[k / 2], mm[k / 2]);
+              epi_split2<SIG>(e, v[i][k], v[i][k + 1], make_float2(os_s[k], os_s[k + 1]), make_float2(os_t[k], os_t[k + 1]), hh[k / 2], mm[k / 2]);
             const size_t so = (size_t)px[i] * e.os_pitch + e.os_coff + c;
             st_bf16_w<W>(e.os_hi + so, hh);
             st_bf16_w<W>(e.os_mid + so, mm);
@@ -194,10 +227,12 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& e, float (&acc0
         }
       }
     }
+    EPI_CLOCK(2);
 #pragma unroll
     for (int i = 0; i + 16 < BN / 2; ++i) { acc0[i] = acc0[i + 16]; acc1[i] = acc1[i + 16]; }
   }
 }
+#undef EPI_CLOCK
 
 // expect_tx + the four operand boxes of one K block, issued by one elected lane of a converged warp
 __device__ __forceinline__ void tma_kblock(uint32_t bar, uint32_t bytes, uint32_t a_hi, uint32_t a_mid, uint32_t b_hi, uint32_t b_mid,
@@ -216,7 +251,9 @@ __device__ __forceinline__ void tma_kblock(uint32_t bar, uint32_t bytes, uint32_
       "r"(c), "r"(x), "r"(y), "r"(n), "r"(k), "r"(n0) : "memory");
 }
 
-template <int ACT, int BN>
+// SIG: EPI_GENERIC runs the epilogue p.staged selects with run-time tests of the chain's parts; any other signature is a staged
+// launch with exactly those parts (epilogue_staged).
+template <int ACT, int BN, int SIG>
 __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_constant__ TmaParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -267,7 +304,9 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
     int j = 0;                                           // tiles processed by this CTA so far, both warpgroups
     if (wg == 1) named_bar_arrive(1, 2 * TM_WG_WARPS * 32);   // warpgroup 0 takes the first turn
 #ifdef MITB_CONV_PHASES
-    long long c0 = 0, c1 = 0, c2 = 0, c3 = 0, c4 = 0, sum[4] = {0, 0, 0, 0}, ntl = 0;
+    long long c0 = 0, c1 = 0, c2 = 0, c3 = 0, c4 = 0, sum[4] = {0, 0, 0, 0}, ntl = 0, ep[3] = {0, 0, 0};
+#else
+    long long* ep = nullptr;
 #endif
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       if (!needed(t)) continue;
@@ -323,15 +362,15 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
         nimg = nimg_t; oy = oy0 + (r >> p.bw_log2); ox = ox0 + (r & (bw - 1));
         return oy < p.Ho && ox < p.Wo && nimg < p.N;
       };
-      if (p.staged) {
+      if (SIG != EPI_GENERIC || p.staged) {
         auto rowm = [&](int r) -> int {
           return p.lin ? ox0 + r : (nimg_t * p.Ho + oy0 + (r >> p.bw_log2)) * p.Wo + ox0 + (r & (bw - 1));
         };
         float* chunk = reinterpret_cast<float*>(epi_smem + wg * EPI_CHUNK_BYTES);
         int* rtab = reinterpret_cast<int*>(epi_smem + 2 * EPI_CHUNK_BYTES) + wg * TC_BM;
-        if (p.e.vec4) epilogue_staged<ACT, BN, 4>(p.e, acc0, acc1, row, n0, chunk, rtab, 3 + wg, rowpix, rowm);
-        else epilogue_staged<ACT, BN, 2>(p.e, acc0, acc1, row, n0, chunk, rtab, 3 + wg, rowpix, rowm);
-      } else {
+        if (p.e.vec4) epilogue_staged<ACT, BN, 4, SIG>(p.e, acc0, acc1, row, n0, chunk, rtab, 3 + wg, rowpix, rowm, ep);
+        else epilogue_staged<ACT, BN, 2, SIG>(p.e, acc0, acc1, row, n0, chunk, rtab, 3 + wg, rowpix, rowm, ep);
+      } else if constexpr (SIG == EPI_GENERIC) {
         epilogue_tile<ACT, BN>(p.e, acc0, row, n0, 0, rowpix);
         epilogue_tile<ACT, BN>(p.e, acc1, 64 + row, n0, 0, rowpix);
       }
@@ -347,6 +386,7 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv_tma_kernel(const __grid_co
       for (int i = 0; i < 4; ++i) atomicAdd(&g_conv_phases[i], (unsigned long long)sum[i]);
       atomicAdd(&g_conv_phases[4], (unsigned long long)ntl);
     }
+    for (int i = 0; i < 3; ++i) atomicAdd(&g_conv_phases[5 + i], (unsigned long long)ep[i]);
 #endif
   } else {
     // =========================== producer warpgroup: its first warp issues four TMA boxes per K block =============
@@ -584,6 +624,38 @@ int choose_bn(int Cout, long mtiles, int nkb, int sms, bool gelu, bool vec2) {
 
 bool g_tma_enabled = true;
 
+// The (activation, epilogue signature) pairs with a conv_tma_kernel of their own: every pair the staged launches of one bench page
+// have (tools/conv_phases.py lists them) - ConvNeXt fc1 (shift, GELU, split) and fc2 (shift, mul1, add1, out), the FFC's spectral
+// and global convs (scale, shift, ReLU, split / + residual and out), the OCR's residual layers (add1, out, split with the next
+// layer's BN + ReLU) and the plain detector / inpainter / OCR convs.  Any other staged launch runs the generic signature.
+#define MITB_EPI_SIGS(X)                                                                \
+  X(ACT_GELU, EPI_SHIFT | EPI_OS)                                                      \
+  X(ACT_GELU, EPI_SHIFT | EPI_OUT)                                                     \
+  X(ACT_NONE, EPI_SHIFT | EPI_MUL1 | EPI_ADD1 | EPI_OUT)                               \
+  X(ACT_NONE, EPI_ADD1 | EPI_OUT | EPI_OS | EPI_OS_AFFINE | EPI_OS_RELU)               \
+  X(ACT_NONE, EPI_SHIFT | EPI_ADD1 | EPI_OUT)                                          \
+  X(ACT_NONE, EPI_SHIFT | EPI_OUT)                                                     \
+  X(ACT_NONE, EPI_OUT)                                                                 \
+  X(ACT_RELU, EPI_SCALE | EPI_SHIFT | EPI_OUT)                                         \
+  X(ACT_RELU, EPI_SCALE | EPI_SHIFT | EPI_OS)                                          \
+  X(ACT_RELU, EPI_SCALE | EPI_SHIFT | EPI_ADD1 | EPI_OUT | EPI_OS)                     \
+  X(ACT_SILU, EPI_SHIFT | EPI_OUT)
+
+template <int A, int SIG> void tma_kernel_attrs() {
+  CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 32, SIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 64, SIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 96, SIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 128, SIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+}
+template <int A, int SIG> void tma_kernel_launch(int BN, int grid, size_t smem, cudaStream_t st, const TmaParams& p) {
+  switch (BN) {
+    case 32: conv_tma_kernel<A, 32, SIG><<<grid, TM_THREADS, smem, st>>>(p); break;
+    case 64: conv_tma_kernel<A, 64, SIG><<<grid, TM_THREADS, smem, st>>>(p); break;
+    case 96: conv_tma_kernel<A, 96, SIG><<<grid, TM_THREADS, smem, st>>>(p); break;
+    default: conv_tma_kernel<A, 128, SIG><<<grid, TM_THREADS, smem, st>>>(p); break;
+  }
+}
+
 // halo a conv needs around its input for reflect padding (zero padding: none)
 void conv_halo(const int8_t* tdy, const int8_t* tdx, int ntaps, int pad, int H, int W, int Ho, int Wo, int sy, int sx, int& pt, int& pb,
                int& pl, int& pr) {
@@ -600,6 +672,30 @@ void conv_halo(const int8_t* tdy, const int8_t* tdx, int ntaps, int pad, int H, 
 }
 
 }  // namespace
+
+int g_epi_specialise = -1;                 // -1: unset, MITB_EPI_GENERIC=1 forces the generic signature
+
+// signature a staged launch with activation instantiation `act` and the chain's parts `sig` runs with
+bool epi_specialise() {
+  if (g_epi_specialise < 0) { const char* ev = getenv("MITB_EPI_GENERIC"); g_epi_specialise = (ev && atoi(ev)) ? 0 : 1; }
+  return g_epi_specialise != 0;
+}
+
+int staged_epi_sig(int act, int sig) {
+  if (!epi_specialise()) return EPI_GENERIC;
+#define MITB_EPI_MATCH(A, S) if (act == (A) && sig == (S)) return S;
+  MITB_EPI_SIGS(MITB_EPI_MATCH)
+#undef MITB_EPI_MATCH
+  return EPI_GENERIC;
+}
+
+int epi_sig_list(int* act, int* sig, int cap) {
+  int n = 0;
+#define MITB_EPI_LIST(A, S) { if (n < cap) { act[n] = A; sig[n] = S; } ++n; }
+  MITB_EPI_SIGS(MITB_EPI_LIST)
+#undef MITB_EPI_LIST
+  return n;
+}
 
 void make_w_tmap(CUtensorMap* m, const uint16_t* base, int kdim, int rows, int bn) {
   const cuuint64_t gdim[2] = {(cuuint64_t)kdim, (cuuint64_t)rows};
@@ -745,13 +841,11 @@ void launch_conv_tma(const ConvOp& op, bool stem, cudaStream_t st) {
   const int num_sms = device_sm_count();
   static PerDeviceOnce tma_attr;
   if (tma_attr.first()) {
-#define MITB_TMA_ATTR(A) \
-    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 96>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-    CUDA_OK(cudaFuncSetAttribute(conv_tma_kernel<A, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    MITB_TMA_ATTR(ACT_NONE) MITB_TMA_ATTR(ACT_RELU) MITB_TMA_ATTR(ACT_GELU) MITB_TMA_ATTR(ACT_SILU) MITB_TMA_ATTR(-1)
-#undef MITB_TMA_ATTR
+    tma_kernel_attrs<ACT_NONE, EPI_GENERIC>(); tma_kernel_attrs<ACT_RELU, EPI_GENERIC>(); tma_kernel_attrs<ACT_GELU, EPI_GENERIC>();
+    tma_kernel_attrs<ACT_SILU, EPI_GENERIC>(); tma_kernel_attrs<-1, EPI_GENERIC>();
+#define MITB_EPI_ATTR(A, S) tma_kernel_attrs<A, S>();
+    MITB_EPI_SIGS(MITB_EPI_ATTR)
+#undef MITB_EPI_ATTR
   }
 
   TmaParams p;
@@ -851,35 +945,36 @@ void launch_conv_tma(const ConvOp& op, bool stem, cudaStream_t st) {
   const long total_tiles = mtiles * (p.npad / BN);
   const int grid = (int)(total_tiles < num_sms ? total_tiles : num_sms);      // persistent: one CTA per SM
   const int act_inst = op.stat_max ? ACT_NONE : (op.act == ACT_NONE || op.act == ACT_RELU || op.act == ACT_GELU || op.act == ACT_SILU) ? op.act : -1;
-  conv_trace(stem ? CK_STEM8 : CK_TMA, BN, 1, p.e.vec2, act_inst, reused, p.staged ? (p.e.vec4 ? 4 : 2) : 0);
-#define MITB_TMA_LAUNCH(A)                                                              \
-  switch (BN) {                                                                        \
-    case 32: conv_tma_kernel<A, 32><<<grid, TM_THREADS, smem, st>>>(p); break;          \
-    case 64: conv_tma_kernel<A, 64><<<grid, TM_THREADS, smem, st>>>(p); break;          \
-    case 96: conv_tma_kernel<A, 96><<<grid, TM_THREADS, smem, st>>>(p); break;          \
-    default: conv_tma_kernel<A, 128><<<grid, TM_THREADS, smem, st>>>(p); break;         \
+  const int sig = p.staged ? staged_epi_sig(act_inst, epi_sig(p.e)) : EPI_GENERIC;
+  conv_trace(stem ? CK_STEM8 : CK_TMA, BN, 1, p.e.vec2, act_inst, reused, p.staged ? (p.e.vec4 ? 4 : 2) : 0, p.staged ? sig : -1);
+  bool launched = false;
+#define MITB_EPI_LAUNCH(A, S) if (!launched && sig == (S) && act_inst == (A)) { tma_kernel_launch<A, S>(BN, grid, smem, st, p); launched = true; }
+  MITB_EPI_SIGS(MITB_EPI_LAUNCH)
+#undef MITB_EPI_LAUNCH
+  if (!launched) {
+    switch (act_inst) {
+      case ACT_NONE: tma_kernel_launch<ACT_NONE, EPI_GENERIC>(BN, grid, smem, st, p); break;
+      case ACT_RELU: tma_kernel_launch<ACT_RELU, EPI_GENERIC>(BN, grid, smem, st, p); break;
+      case ACT_GELU: tma_kernel_launch<ACT_GELU, EPI_GENERIC>(BN, grid, smem, st, p); break;
+      case ACT_SILU: tma_kernel_launch<ACT_SILU, EPI_GENERIC>(BN, grid, smem, st, p); break;
+      default: tma_kernel_launch<-1, EPI_GENERIC>(BN, grid, smem, st, p); break;
+    }
   }
-  switch (op.stat_max ? ACT_NONE : op.act) {
-    case ACT_NONE: MITB_TMA_LAUNCH(ACT_NONE); break;
-    case ACT_RELU: MITB_TMA_LAUNCH(ACT_RELU); break;
-    case ACT_GELU: MITB_TMA_LAUNCH(ACT_GELU); break;
-    case ACT_SILU: MITB_TMA_LAUNCH(ACT_SILU); break;
-    default: MITB_TMA_LAUNCH(-1); break;
-  }
-#undef MITB_TMA_LAUNCH
   count_launch();
   g_key_epoch = g_launch_epoch;
   CUDA_OK(cudaGetLastError());
 #ifdef MITB_CONV_PHASES
   {
-    unsigned long long ph[5];
+    unsigned long long ph[N_PHASES];
     CUDA_OK(cudaStreamSynchronize(st));
     CUDA_OK(cudaMemcpyFromSymbol(ph, g_conv_phases, sizeof(ph)));
-    const unsigned long long zero[5] = {0, 0, 0, 0, 0};
+    const unsigned long long zero[N_PHASES] = {};
     CUDA_OK(cudaMemcpyToSymbol(g_conv_phases, zero, sizeof(zero)));
     const int K = op.wt.ntaps * C + (two ? op.seg2.ntaps * op.seg2.C : 0);      // the GEMM shape tools/layer_times.py reports
-    fprintf(stderr, "mitb_conv_phases M %d K %d N %d BN %d nkb %d ctas %d tiles %llu first_wait %llu main %llu wgmma_wait %llu epilogue %llu\n",
-            N * op.Ho * op.Wo, K, op.out.C, BN, p.nkb, grid, ph[4], ph[0], ph[1], ph[2], ph[3]);
+    fprintf(stderr, "mitb_conv_phases M %d K %d N %d BN %d nkb %d ctas %d tiles %llu first_wait %llu main %llu wgmma_wait %llu epilogue %llu"
+            " epi_chunk %llu epi_vec %llu epi_rows %llu act %d parts %d sig %d staged %d\n",
+            N * op.Ho * op.Wo, K, op.out.C, BN, p.nkb, grid, ph[4], ph[0], ph[1], ph[2], ph[3], ph[5] / 128, ph[6] / 128, ph[7] / 128,
+            act_inst, epi_sig(p.e), sig, p.staged ? (p.e.vec4 ? 4 : 2) : 0);
   }
 #endif
 }

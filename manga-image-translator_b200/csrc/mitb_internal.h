@@ -154,14 +154,28 @@ void launch_conv_tma(const ConvOp& op, bool stem, cudaStream_t st);   // stem: a
 // weight tensor map (conv_tma.cu): bf16 [rows][kdim] K-major, box {64 k, bn}, 128-byte swizzle; rows beyond `rows` are zero filled
 void make_w_tmap(CUtensorMap* m, const uint16_t* base, int kdim, int rows, int bn);
 // Host-side record of what launch_conv() ran (test hook mitb_test_conv): null by default, and nothing is recorded then.
-struct ConvTrace { int kernel = 0, bn = 0, splits = 1, vec2 = -1, tma_act = -2, split_reused = 0, convs = 0, staged = -1; };
+// Epilogue signature: which parts of the fused conv epilogue a launch has (tc_common.cuh: epi_sig).  EPI_GENERIC tests every
+// part at run time.
+enum EpiSig : int {
+  EPI_ADD0 = MITB_EPI_ADD0, EPI_SCALE = MITB_EPI_SCALE, EPI_SHIFT = MITB_EPI_SHIFT, EPI_MUL1 = MITB_EPI_MUL1, EPI_ADD1 = MITB_EPI_ADD1,
+  EPI_OUT = MITB_EPI_OUT, EPI_OS = MITB_EPI_OS, EPI_OS_AFFINE = MITB_EPI_OS_AFFINE, EPI_OS_RELU = MITB_EPI_OS_RELU, EPI_GENERIC = MITB_EPI_GENERIC
+};
+// epi_sig: the staged epilogue's signature (EpiSig, tc_common.cuh) that ran, -1 for other epilogues and kernels.
+struct ConvTrace { int kernel = 0, bn = 0, splits = 1, vec2 = -1, tma_act = -2, split_reused = 0, convs = 0, staged = -1, epi_sig = -1; };
 extern ConvTrace* g_conv_trace;
-inline void conv_trace(int kernel, int bn, int splits, int vec2, int tma_act, bool reused, int staged = -1) {
+inline void conv_trace(int kernel, int bn, int splits, int vec2, int tma_act, bool reused, int staged = -1, int epi_sig = -1) {
   if (!g_conv_trace) return;
   ConvTrace& t = *g_conv_trace;
   t.kernel = kernel; t.bn = bn; t.splits = splits; t.vec2 = vec2; t.tma_act = tma_act; t.split_reused += reused ? 1 : 0; ++t.convs;
-  t.staged = staged;
+  t.staged = staged; t.epi_sig = epi_sig;
 }
+// TMA conv epilogue signatures (conv_tma.cu): g_epi_specialise 1 runs a staged launch on its signature's own kernel where one is
+// instantiated, 0 on the generic one; -1 until epi_specialise() reads MITB_EPI_GENERIC (=1: 0).  Test hook mitb_set_epi_specialise.
+// staged_epi_sig() is the signature a staged launch runs with.
+extern int g_epi_specialise;
+bool epi_specialise();
+int staged_epi_sig(int act, int sig);
+int epi_sig_list(int* act, int* sig, int cap);     // the (activation, signature) pairs with a kernel of their own; returns their count
 extern int g_conv_force_bn;                // non-zero: the TMA kernel's N tile (must be one of choose_bn's candidates); test hook only
 bool conv_tma_bn_candidate(int Cout, int bn);
 bool conv_tc_enabled();

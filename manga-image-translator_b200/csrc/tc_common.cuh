@@ -224,22 +224,38 @@ __device__ __forceinline__ void stat_merge(float& am, float& as, int& ai, float 
   am = m;
 }
 
+// Epilogue signature (EpiSig, mitb_internal.h) of a launch: a bitmask that a kernel can take as a template parameter
+// (epilogue_staged declares, loads and tests only what its signature has).
+inline int epi_sig(const EpiParams& e) {
+  return (e.add0 ? EPI_ADD0 : 0) | (e.scale ? EPI_SCALE : 0) | (e.shift ? EPI_SHIFT : 0) | (e.mul1 ? EPI_MUL1 : 0) | (e.add1 ? EPI_ADD1 : 0) |
+         (e.out ? EPI_OUT : 0) | (e.os_hi ? EPI_OS : 0) | (e.os_hi && e.os_scale ? EPI_OS_AFFINE : 0) |
+         (e.os_hi && e.os_scale && e.os_relu ? EPI_OS_RELU : 0);
+}
+// does a launch of signature SIG have part BIT (rt: the run-time test, used by EPI_GENERIC only)
+template <int SIG, int BIT> __device__ __forceinline__ bool epi_has(bool rt) {
+  if constexpr (SIG == EPI_GENERIC) return rt;
+  else return (SIG & BIT) != 0;
+}
+
 // The fused elementwise chain of two adjacent columns, v = acc (+add0) ; v = v*scale+shift ; act ; *mul1 ; +add1, and the split of
 // its result into the consumer's bf16 hi / mid operands (after the consumer's prologue os_scale / os_shift / os_relu).  Every
 // two-column epilogue calls these, so the fp32 operations and their order, which the outputs' bits depend on, live in one place.
-template <int ACT>
+// The products and sums are explicitly rounded: a signature with both scale and shift (or mul1 and add1) must not contract them
+// into one FMA, so that every signature computes the bits of the generic chain.
+template <int ACT, int SIG = EPI_GENERIC>
 __device__ __forceinline__ void epi_chain2(const EpiParams& e, float& v0, float& v1, float2 a0, float2 sc, float2 sh, float2 m1, float2 a1) {
-  if (e.add0) { v0 += a0.x; v1 += a0.y; }
-  if (e.scale) { v0 *= sc.x; v1 *= sc.y; }
-  if (e.shift) { v0 += sh.x; v1 += sh.y; }
+  if (epi_has<SIG, EPI_ADD0>(e.add0)) { v0 = __fadd_rn(v0, a0.x); v1 = __fadd_rn(v1, a0.y); }
+  if (epi_has<SIG, EPI_SCALE>(e.scale)) { v0 = __fmul_rn(v0, sc.x); v1 = __fmul_rn(v1, sc.y); }
+  if (epi_has<SIG, EPI_SHIFT>(e.shift)) { v0 = __fadd_rn(v0, sh.x); v1 = __fadd_rn(v1, sh.y); }
   v0 = act_t<ACT>(v0, e.act); v1 = act_t<ACT>(v1, e.act);
-  if (e.mul1) { v0 *= m1.x; v1 *= m1.y; }
-  if (e.add1) { v0 += a1.x; v1 += a1.y; }
+  if (epi_has<SIG, EPI_MUL1>(e.mul1)) { v0 = __fmul_rn(v0, m1.x); v1 = __fmul_rn(v1, m1.y); }
+  if (epi_has<SIG, EPI_ADD1>(e.add1)) { v0 = __fadd_rn(v0, a1.x); v1 = __fadd_rn(v1, a1.y); }
 }
+template <int SIG = EPI_GENERIC>
 __device__ __forceinline__ void epi_split2(const EpiParams& e, float v0, float v1, float2 s, float2 t, uint32_t& hi, uint32_t& mid) {
-  if (e.os_scale) {
+  if (epi_has<SIG, EPI_OS_AFFINE>(e.os_scale)) {
     v0 = fmaf(v0, s.x, t.x); v1 = fmaf(v1, s.y, t.y);
-    if (e.os_relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+    if (epi_has<SIG, EPI_OS_RELU>(e.os_relu)) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
   }
   split2(v0, v1, hi, mid);
 }

@@ -22,7 +22,8 @@ static_assert(offsetof(mitb_test_conv_desc, N) == 8 && offsetof(mitb_test_conv_d
               "test hook descriptor layout");
 static_assert(offsetof(mitb_test_conv_info, bn) == 4 && offsetof(mitb_test_conv_info, splits) == 8 && offsetof(mitb_test_conv_info, vec2) == 12 &&
               offsetof(mitb_test_conv_info, tma_act) == 16 && offsetof(mitb_test_conv_info, split_reused) == 20 &&
-              offsetof(mitb_test_conv_info, convs) == 24 && offsetof(mitb_test_conv_info, staged) == 28 && sizeof(mitb_test_conv_info) == 32, "test hook info layout");
+              offsetof(mitb_test_conv_info, convs) == 24 && offsetof(mitb_test_conv_info, staged) == 28 &&
+              offsetof(mitb_test_conv_info, epi_sig) == 32 && sizeof(mitb_test_conv_info) == 36, "test hook info layout");
 
 namespace {
 
@@ -154,7 +155,7 @@ int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* d, mitb_test_conv_i
     MITB_CHECK(!d->force_bn || on_tma, "test_conv: force_bn needs the TMA-fed kernel (kernel %d)", tr.kernel);
     memset(info, 0, sizeof(*info));
     info->kernel = tr.kernel; info->bn = tr.bn; info->splits = tr.splits; info->vec2 = tr.vec2; info->tma_act = tr.tma_act;
-    info->split_reused = tr.split_reused; info->convs = tr.convs; info->staged = tr.staged;
+    info->split_reused = tr.split_reused; info->convs = tr.convs; info->staged = tr.staged; info->epi_sig = tr.epi_sig;
     return 0;
   } catch (const std::exception& ex) {
     ctx->c.err = ex.what();
@@ -162,5 +163,15 @@ int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* d, mitb_test_conv_i
     return 2;
   }
 }
+
+int mitb_set_epi_specialise(int on) {
+  const int prev = epi_specialise() ? 1 : 0;
+  g_epi_specialise = on ? 1 : 0;
+  return prev;
+}
+
+int mitb_test_epi_signature(int act, int sig) { return staged_epi_sig(act, sig); }
+
+int mitb_test_epi_signatures(int* act, int* sig, int cap) { return epi_sig_list(act, sig, cap); }
 
 }  // extern "C"

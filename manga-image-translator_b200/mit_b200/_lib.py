@@ -44,7 +44,7 @@ class MitbTestConvDesc(C.Structure):
 
 
 class MitbTestConvInfo(C.Structure):
-    _fields_ = _ints("kernel", "bn", "splits", "vec2", "tma_act", "split_reused", "convs", "staged")
+    _fields_ = _ints("kernel", "bn", "splits", "vec2", "tma_act", "split_reused", "convs", "staged", "epi_sig")
 
 
 class MitbError(RuntimeError):
@@ -110,6 +110,9 @@ SIGNATURES = {
     "mitb_op_dilate_se": (I, [P, P, I, I, P, I, P, P]),
     "mitb_test_conv": (I, [P, C.POINTER(MitbTestConvDesc), C.POINTER(MitbTestConvInfo), P]),
     "mitb_test_struct_sizes": (I, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "mitb_set_epi_specialise": (I, [I]),
+    "mitb_test_epi_signature": (I, [I, I]),
+    "mitb_test_epi_signatures": (I, [C.POINTER(C.c_int), C.POINTER(C.c_int), I]),
 }
 
 
