@@ -283,6 +283,20 @@ typedef struct {             /* what the last conv launch of the call ran */
 int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* desc, mitb_test_conv_info* info, void* stream);
 int mitb_test_struct_sizes(int* desc_bytes, int* info_bytes);
 
+/* The OCR's vocabulary head on its own, built and run as mitb_ocr_forward builds it: logits = x wt^T + bias with log-softmax and
+ * argmax fused into the GEMM's epilogue (the logits are never stored), then the merge of the per-block partials.  x fp32 [n*t][c]
+ * (c a multiple of 4), wt [v][c], bias [v] (NULL: none), path MITB_TEST_PATH_*.  idx int32 / logprob fp32 [n*t]: the first maximal
+ * column of each row and its log-softmax value.
+ * Partials: *nblk blocks per row, row r's block b at [r * nblk + b] of pmax (the block's max logit), psum (sum over the block of
+ * exp(logit - block max)) and pidx (first column holding the block max); a block with no column < v holds (-inf, 0, INT32_MAX).
+ * Tensor-core kernels (N tile bn, info->bn): blocks 2 i and 2 i + 1 are columns [i bn, i bn + h) and [i bn + h, (i + 1) bn) with
+ * h = 16 * ceil(bn / 32).  SIMT kernel: block b is columns [128 b, 128 b + 128).  pmax / psum / pidx NULL: internal buffers; else
+ * device buffers of cap >= n * t * nblk elements each, which the kernels write in place (nothing past n * t * nblk).  Fills *nblk and
+ * *info (the conv launch's kernel and N tile). */
+int mitb_test_vocab_head(mitb_ctx* ctx, const float* x, int n, int t, int c, const float* wt, const float* bias, int v, int path,
+                         int32_t* idx, float* logprob, float* pmax, float* psum, int32_t* pidx, long long cap, int32_t* nblk,
+                         mitb_test_conv_info* info, void* stream);
+
 /* Epilogue signatures of the TMA conv kernel's staged epilogue: which parts of the fused chain a launch has.  A staged launch whose
  * (activation, signature) pair has a kernel of its own runs it; any other runs MITB_EPI_GENERIC, which tests every part at run time. */
 #define MITB_EPI_ADD0 1

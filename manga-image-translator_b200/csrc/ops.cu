@@ -423,49 +423,68 @@ void launch_affine_act(const View& in, const View& out, const float* scale, cons
 
 // ---------------------------------------------------------------------------------------------------
 // OCR self-attention core (model_48px_ctc.py:263-269 -> F.multi_head_attention_forward): one CTA per
-// (line, head); K and V of that head staged in shared memory (stride hd+1), one warp per query row,
-// softmax(q.k / sqrt(hd)) v with no padding mask.
-// gridDim.y row blocks per (line, head): each CTA re-stages K/V (L2 resident) and takes every gridDim.y-th group of query rows,
-// so the 128 (line, head) pairs of a 16-line chunk fill all SMs (132 on an H100) several CTAs deep instead of 128 SMs one CTA deep.
+// (line, head), one warp per query row, softmax(q.k / sqrt(hd)) v with no padding mask.
+// gridDim.y row blocks per (line, head): each CTA takes every gridDim.y-th group of query rows, so the 128 (line, head) pairs of
+// a 16-line chunk fill all SMs (132 on an H100) several CTAs deep instead of 128 SMs one CTA deep.
+// Keys and values stream through shared memory in blocks of AT_KB (stride hd+1), so the footprint does not grow with T: each row
+// keeps a running max and sum, and its running output (Os, one entry per lane-owned dimension) is rescaled by exp(old max - new
+// max) whenever a block raises the max.  With T <= AT_KB this is the one-pass softmax bit for bit.
+constexpr int AT_KB = 64;
 __global__ void attention_kernel(const float* qk, const float* v, float* out, int T, int heads, int hd, float scale) {
   extern __shared__ float sm[];
   const int D = heads * hd;
   const int n = blockIdx.x / heads, h = blockIdx.x % heads;
   const int ld = hd + 1;
-  float* Ks = sm; float* Vs = Ks + (size_t)T * ld;
-  float* Ps = Vs + (size_t)T * ld;               // [nwarps][T] probabilities
-  float* Qs = Ps + (size_t)(blockDim.x >> 5) * T; // [nwarps][hd]
-  for (int i = threadIdx.x; i < T * hd; i += blockDim.x) {
-    const int t = i / hd, d = i % hd;
-    Ks[t * ld + d] = qk[((size_t)n * T + t) * 2 * D + D + h * hd + d];
-    Vs[t * ld + d] = v[((size_t)n * T + t) * D + h * hd + d];
-  }
-  __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  float* P = Ps + (size_t)warp * T; float* Q = Qs + warp * hd;
-  for (int t = blockIdx.y * nw + warp; t < T; t += nw * gridDim.y) {
-    for (int d = lane; d < hd; d += 32) Q[d] = qk[((size_t)n * T + t) * 2 * D + h * hd + d];
-    __syncwarp();
-    float mx = -INFINITY;
-    for (int j = lane; j < T; j += 32) {
-      float s = 0.f;
-      for (int d = 0; d < hd; ++d) s = fmaf(Q[d], Ks[j * ld + d], s);
-      s *= scale; P[j] = s; mx = fmaxf(mx, s);
-    }
+  float* Ks = sm; float* Vs = Ks + AT_KB * ld;
+  float* Ps = Vs + AT_KB * ld;                   // [nwarps][AT_KB] probabilities of the current key block
+  float* Qs = Ps + nw * AT_KB;                   // [nwarps][hd]
+  float* Os = Qs + nw * hd;                      // [nwarps][hd] running outputs
+  float* P = Ps + warp * AT_KB; float* Q = Qs + warp * hd; float* O = Os + warp * hd;
+  // the row-group loop is uniform over the CTA (every warp meets the key-block barriers); a warp past T only helps stage
+  for (int t0 = blockIdx.y * nw; t0 < T; t0 += nw * gridDim.y) {
+    const int t = t0 + warp;
+    const bool row = t < T;
+    if (row)
+      for (int d = lane; d < hd; d += 32) { Q[d] = qk[((size_t)n * T + t) * 2 * D + h * hd + d]; O[d] = 0.f; }
+    float mx = -INFINITY, sum = 0.f;
+    for (int j0 = 0; j0 < T; j0 += AT_KB) {
+      const int nk = min(AT_KB, T - j0);
+      __syncthreads();                           // the previous block's readers are done
+      for (int i = threadIdx.x; i < nk * hd; i += blockDim.x) {
+        const int j = i / hd, d = i % hd;
+        Ks[j * ld + d] = qk[((size_t)n * T + j0 + j) * 2 * D + D + h * hd + d];
+        Vs[j * ld + d] = v[((size_t)n * T + j0 + j) * D + h * hd + d];
+      }
+      __syncthreads();
+      if (!row) continue;
+      float bm = -INFINITY;
+      for (int j = lane; j < nk; j += 32) {
+        float s = 0.f;
+        for (int d = 0; d < hd; ++d) s = fmaf(Q[d], Ks[j * ld + d], s);
+        s *= scale; P[j] = s; bm = fmaxf(bm, s);
+      }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    float sum = 0.f;
-    for (int j = lane; j < T; j += 32) { float e = expf(P[j] - mx); P[j] = e; sum += e; }
+      for (int o = 16; o > 0; o >>= 1) bm = fmaxf(bm, __shfl_xor_sync(0xffffffffu, bm, o));
+      const float m = fmaxf(mx, bm);
+      float bs = 0.f;
+      for (int j = lane; j < nk; j += 32) { float e = expf(P[j] - m); P[j] = e; bs += e; }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    __syncwarp();
-    const float inv = 1.f / sum;
-    for (int d = lane; d < hd; d += 32) {
-      float a = 0.f;
-      for (int j = 0; j < T; ++j) a = fmaf(P[j], Vs[j * ld + d], a);
-      out[((size_t)n * T + t) * D + h * hd + d] = a * inv;
+      for (int o = 16; o > 0; o >>= 1) bs += __shfl_xor_sync(0xffffffffu, bs, o);
+      const float c = expf(mx - m);              // 0 for the first block
+      sum = sum * c + bs; mx = m;
+      __syncwarp();
+      for (int d = lane; d < hd; d += 32) {
+        float a = 0.f;
+        for (int j = 0; j < nk; ++j) a = fmaf(P[j], Vs[j * ld + d], a);
+        O[d] = O[d] * c + a;
+      }
+      __syncwarp();
     }
-    __syncwarp();
+    if (row) {
+      const float inv = 1.f / sum;
+      for (int d = lane; d < hd; d += 32) out[((size_t)n * T + t) * D + h * hd + d] = O[d] * inv;
+    }
   }
 }
 
@@ -559,9 +578,9 @@ void launch_attention(const float* qk, const float* v, float* out, int N, int T,
       return;
     }
   }
-  const int threads = 256;
-  const size_t smem = ((size_t)2 * T * (hd + 1) + (size_t)(threads / 32) * T + (size_t)(threads / 32) * hd) * sizeof(float);
-  MITB_CHECK(smem <= 200 * 1024, "attention: sequence too long (T=%d)", T);
+  const int threads = 256, nw = threads / 32;
+  const size_t smem = ((size_t)2 * AT_KB * (hd + 1) + (size_t)nw * AT_KB + (size_t)2 * nw * hd) * sizeof(float);
+  MITB_CHECK(hd >= 1 && smem <= 200 * 1024, "attention: head_dim %d unsupported", hd);
   static PerDeviceOnce attr_set;
   if (attr_set.first()) CUDA_OK(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   ProfScope ps("attention", 4.0 * N * heads * (double)T * T * hd, 16.0 * N * T * heads * hd, st);

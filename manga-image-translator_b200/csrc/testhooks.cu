@@ -1,6 +1,7 @@
 // Test hooks of include/mitb.h (not for production use): one fully described convolution through launch_conv(), so that tests
 // can reach every option of the fused conv epilogue (ConvOp in mitb_internal.h) on every kernel path and compare it with an
-// independent reference.  Host code only: the kernels are the ones the networks run.
+// independent reference, and the OCR's vocabulary head (GEMM + fused log-softmax / argmax) with its row-stat partials.  Host
+// code only: the kernels are the ones the networks run.
 #include <stddef.h>
 #include <string.h>
 #include "exec.h"
@@ -32,6 +33,19 @@ struct HookGuard {
   bool tc = conv_tc_enabled(), tma = conv_tma_enabled();
   ~HookGuard() { conv_tc_set_enabled(tc); conv_tma_set_enabled(tma); g_conv_trace = nullptr; g_conv_force_bn = 0; }
 };
+
+// the process-wide kernel switches of a MITB_TEST_PATH_*
+void set_path(int path) {
+  if (path == MITB_TEST_PATH_SIMT) conv_tc_set_enabled(false);
+  if (path == MITB_TEST_PATH_GATHER) conv_tma_set_enabled(false);
+  if (path == MITB_TEST_PATH_TMA || path == MITB_TEST_PATH_AUTO) { conv_tc_set_enabled(true); conv_tma_set_enabled(true); }
+}
+
+void fill_info(mitb_test_conv_info* info, const ConvTrace& tr) {
+  memset(info, 0, sizeof(*info));
+  info->kernel = tr.kernel; info->bn = tr.bn; info->splits = tr.splits; info->vec2 = tr.vec2; info->tma_act = tr.tma_act;
+  info->split_reused = tr.split_reused; info->convs = tr.convs; info->staged = tr.staged; info->epi_sig = tr.epi_sig;
+}
 
 void check_align(const void* p, unsigned a, const char* what) {
   MITB_CHECK(((uintptr_t)p & (a - 1)) == 0, "test_conv: %s must be %u-byte aligned (unaligned slices go through cs / coff)", what, a);
@@ -140,9 +154,7 @@ int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* d, mitb_test_conv_i
     // a fused op on any other kernel would dereference the shape-only views
     MITB_CHECK(!fused || conv_tma_capable(op), "test_conv: this op cannot run on the TMA-fed kernel");
 
-    if (d->path == MITB_TEST_PATH_SIMT) conv_tc_set_enabled(false);
-    if (d->path == MITB_TEST_PATH_GATHER) conv_tma_set_enabled(false);
-    if (d->path == MITB_TEST_PATH_TMA || d->path == MITB_TEST_PATH_AUTO) { conv_tc_set_enabled(true); conv_tma_set_enabled(true); }
+    set_path(d->path);
     ConvTrace tr;
     g_conv_trace = &tr; g_conv_force_bn = d->force_bn;
     CUDA_OK(cudaStreamSynchronize(st));                     // weight copies ready
@@ -153,9 +165,60 @@ int mitb_test_conv(mitb_ctx* ctx, const mitb_test_conv_desc* d, mitb_test_conv_i
     const bool on_tma = tr.kernel == CK_TMA || tr.kernel == CK_STEM8;
     MITB_CHECK(d->path != MITB_TEST_PATH_TMA || on_tma, "test_conv: the op did not run on the TMA-fed kernel (kernel %d)", tr.kernel);
     MITB_CHECK(!d->force_bn || on_tma, "test_conv: force_bn needs the TMA-fed kernel (kernel %d)", tr.kernel);
-    memset(info, 0, sizeof(*info));
-    info->kernel = tr.kernel; info->bn = tr.bn; info->splits = tr.splits; info->vec2 = tr.vec2; info->tma_act = tr.tma_act;
-    info->split_reused = tr.split_reused; info->convs = tr.convs; info->staged = tr.staged; info->epi_sig = tr.epi_sig;
+    fill_info(info, tr);
+    return 0;
+  } catch (const std::exception& ex) {
+    ctx->c.err = ex.what();
+    cudaGetLastError();
+    return 2;
+  }
+}
+
+int mitb_test_vocab_head(mitb_ctx* ctx, const float* x, int n, int t, int c, const float* wt, const float* bias, int v, int path,
+                         int32_t* idx, float* logprob, float* pmax, float* psum, int32_t* pidx, long long cap, int32_t* nblk,
+                         mitb_test_conv_info* info, void* stream) {
+  if (!ctx) return 1;
+  HookGuard guard;
+  try {
+    CUDA_OK(cudaSetDevice(ctx->c.device));
+    cudaStream_t st = (cudaStream_t)stream;
+    MITB_CHECK(path >= MITB_TEST_PATH_AUTO && path <= MITB_TEST_PATH_TMA, "test_vocab_head: bad path %d", path);
+    MITB_CHECK(n > 0 && t > 0 && c > 0 && c % 4 == 0 && v > 0, "test_vocab_head: bad shape");
+    MITB_CHECK(x && wt && idx && logprob && nblk && info, "test_vocab_head: null buffer");
+    MITB_CHECK(!pmax == !psum && !pmax == !pidx, "test_vocab_head: pmax, psum and pidx go together");
+    check_align(x, 16, "x");
+
+    // char_pred as ocr_build loads it
+    DevBlob blob;
+    Weights W;
+    W.t["w"] = mitb_tensor{"w", wt, 2, {v, c}};
+    if (bias) W.t["b"] = mitb_tensor{"b", bias, 1, {v}};
+    Loader L{W, blob, st};
+    ConvW cw = L.conv("w", 0, 0);
+    if (bias) cw.shift = L.vec("b");
+
+    // the op as ocr_run makes it, its stat layout read after the path switches are set
+    View in; in.p = const_cast<float*>(x); in.N = n; in.H = 1; in.W = t; in.C = c; in.cs = c; in.coff = 0;
+    View out = in; out.p = nullptr; out.C = v; out.cs = v;
+    ConvOp op = Exec::op_from(cw, in, out);
+    set_path(path);
+    const int nb = conv_stat_blocks(op);
+    const long long need = (long long)n * t * nb;
+    if (pmax) MITB_CHECK(cap >= need, "test_vocab_head: partials need %lld elements, cap %lld", need, cap);
+    else { pmax = blob.alloc_f(need); psum = blob.alloc_f(need); pidx = (int32_t*)blob.alloc_f(need); }
+    op.stat_max = pmax; op.stat_sum = psum; op.stat_idx = pidx; op.stat_ld = nb;
+
+    ConvTrace tr;
+    g_conv_trace = &tr;
+    CUDA_OK(cudaStreamSynchronize(st));                     // weight copies ready
+    ++g_launch_epoch;
+    launch_conv(op, st);
+    launch_rowstat_final(pmax, psum, pidx, n * t, nb, idx, logprob, st);
+    CUDA_OK(cudaStreamSynchronize(st));
+    const bool on_tma = tr.kernel == CK_TMA;
+    MITB_CHECK(path != MITB_TEST_PATH_TMA || on_tma, "test_vocab_head: the op did not run on the TMA-fed kernel (kernel %d)", tr.kernel);
+    fill_info(info, tr);
+    *nblk = nb;
     return 0;
   } catch (const std::exception& ex) {
     ctx->c.err = ex.what();

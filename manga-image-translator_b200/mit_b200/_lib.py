@@ -110,6 +110,7 @@ SIGNATURES = {
     "mitb_op_dilate_se": (I, [P, P, I, I, P, I, P, P]),
     "mitb_test_conv": (I, [P, C.POINTER(MitbTestConvDesc), C.POINTER(MitbTestConvInfo), P]),
     "mitb_test_struct_sizes": (I, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "mitb_test_vocab_head": (I, [P, P, I, I, I, P, P, I, I, P, P, P, P, P, LL, C.POINTER(C.c_int32), C.POINTER(MitbTestConvInfo), P]),
     "mitb_set_epi_specialise": (I, [I]),
     "mitb_test_epi_signature": (I, [I, I]),
     "mitb_test_epi_signatures": (I, [C.POINTER(C.c_int), C.POINTER(C.c_int), I]),

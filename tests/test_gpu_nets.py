@@ -87,8 +87,9 @@ def test_ocr_golden_and_oracle(eng, golden_dir):
         assert [(b, c[0]) for b, l in enumerate(dec) for c in l] == [(int(r[0]), int(r[1])) for r in g["decoded"]]
     idx8, lp8, col8 = eng.ocr_forward(torch.from_numpy(img))
     assert torch.equal(idx8, idx) and _err(lp8, lp.cpu()) < 1e-6
-    # other widths / chunk sizes against the oracle, incl. a full chunk of 16
-    for n, wp in ((1, 143), (5, 331), (16, 263)):
+    # other widths / chunk sizes against the oracle, incl. a full chunk of 16 and a line too wide for attention held in shared
+    # memory whole (T = 599)
+    for n, wp in ((1, 143), (5, 331), (16, 263), (1, 2400)):
         _, x = cases.ocr_case(n, wp, seed=100 + wp)
         idx, lp, col = eng.ocr_forward(x)
         o_idx, o_lp, o_col = nets.ocr_top1(sd, x)
