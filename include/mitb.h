@@ -297,6 +297,42 @@ int mitb_test_vocab_head(mitb_ctx* ctx, const float* x, int n, int t, int c, con
                          int32_t* idx, float* logprob, float* pmax, float* psum, int32_t* pidx, long long cap, int32_t* nblk,
                          mitb_test_conv_info* info, void* stream);
 
+/* One real 2-D FFT (torch.fft.rfftn / irfftn over (h, w), norm='ortho') launched as LaMa's FFC layers launch it, on either
+ * implementation, for tests that pin both kernels against a float64 reference.  Its layout is fixed like the conv hook's ("@N").
+ * Planar (the generic path, any 1 <= h, w <= 4096): in, out and add are contiguous planes (cs = C, coff = 0): forward in [N*C][h][w]
+ * -> out [N*2C][h][w/2+1] (re / im planes interleaved per channel); inverse the other way round, + add [N*C][h][w].
+ * NHWC (the fused path, h and w {2,3,5}-smooth and <= 512, C even): forward in = channels [coff, coff + C) of [N][h][w][cs] ->
+ * out dense fp32 [N][h][w/2+1][2C] and / or out_sv dense bf16 hi / mid [N][h][w/2+1][2C] (C = 2C, coff 0, Hp = h, Wp = w/2+1, no
+ * halo); inverse in = channels [coff, coff + 2C) of [N][h][w/2+1][cs] -> out channels [coff, coff + C) of [N][h][w][cs] and / or
+ * out_sv channels [coff, coff + C) of [N][h][w][C_sv] (+ add, channels [coff, coff + C) of [N][h][w][cs]).  The planar field of
+ * the views is ignored. */
+#define MITB_TEST_FFT_PLANAR 0
+#define MITB_TEST_FFT_NHWC 1
+
+typedef struct {
+  int32_t impl, inverse;     /* @0 MITB_TEST_FFT_*; 0 rfft2, 1 irfft2 */
+  int32_t N, h, w, C;        /* @8 images, transform size, real channels */
+  mitb_test_view in;         /* @24 */
+  mitb_test_view out;        /* @48 fp32 output; p NULL only on NHWC with out_sv */
+  mitb_test_split out_sv;    /* @72 NHWC bf16 hi / mid output (hi NULL: none) */
+  mitb_test_view add;        /* @112 inverse residual (p NULL: none) */
+  int32_t force_plain, reserved;   /* @136 NHWC: plain loads wherever the TMA box would have run */
+} mitb_test_fft_desc;        /* 144 bytes */
+
+typedef struct {             /* what the call ran */
+  int32_t h_nst;             /* @0 stages of the length-h plan */
+  int32_t h_radix[16];       /* @4 its radices, first stage first */
+  int32_t w_nst;             /* @68 */
+  int32_t w_radix[16];       /* @72 */
+  int32_t rows_tma, rows_box_rows;   /* @136 NHWC row pass: TMA box (1) or plain loads (0), rows per box (0: plain); -1 planar */
+  int32_t cols_tma, cols_box_rows;   /* @144 NHWC column pass */
+  int32_t P, CB;             /* @152 planar: row pairs per row-pass CTA, columns per column-pass CTA; 0 NHWC */
+} mitb_test_fft_info;        /* 160 bytes */
+
+/* Runs the transform on `stream`, synchronises, fills *info.  Error (non-zero) for a bad descriptor or a shape the implementation
+ * does not take.  Scratch is allocated per call. */
+int mitb_test_fft(mitb_ctx* ctx, const mitb_test_fft_desc* desc, mitb_test_fft_info* info, void* stream);
+
 /* Epilogue signatures of the TMA conv kernel's staged epilogue: which parts of the fused chain a launch has.  A staged launch whose
  * (activation, signature) pair has a kernel of its own runs it; any other runs MITB_EPI_GENERIC, which tests every part at run time. */
 #define MITB_EPI_ADD0 1

@@ -21,6 +21,8 @@ constexpr int kMaxStages = 16;
 struct FftDev { int n, nstages; int radix[kMaxStages]; const float2* tw; };
 struct FftPlan { FftDev dev; };
 
+FftTrace* g_fft_trace = nullptr;
+
 static std::mutex g_plan_mu;
 static std::map<std::pair<int, int>, FftPlan*> g_plans;    // (device, n)
 
@@ -225,6 +227,17 @@ static const float* planar_base(const View& v, int* planes) {
   return v.p + (size_t)v.coff * v.H * v.W;
 }
 
+// test hook record: the two plans' radix sequences and the batching of the row and column passes
+static void fft_trace(const FftPlan* ph, const FftPlan* pw, int P, int CB) {
+  if (!g_fft_trace) return;
+  FftTrace& t = *g_fft_trace;
+  t = FftTrace();
+  t.h_nst = ph->dev.nstages; t.w_nst = pw->dev.nstages;
+  for (int s = 0; s < ph->dev.nstages; ++s) t.h_radix[s] = ph->dev.radix[s];
+  for (int s = 0; s < pw->dev.nstages; ++s) t.w_radix[s] = pw->dev.radix[s];
+  t.P = P; t.CB = CB;
+}
+
 static int pick_batch(int n, int per_elem_bytes, int want) {
   int b = want;
   while (b > 1 && (size_t)2 * b * (n | 1) * per_elem_bytes > 96 * 1024) b >>= 1;
@@ -242,6 +255,7 @@ void launch_rfft2(const View& in, const View& spec, float2* tmp, cudaStream_t st
   FftPlan* pw = fft_plan_get(w); FftPlan* ph = fft_plan_get(h);
   const int P = pick_batch(w, 8, 8), CB = pick_batch(h, 8, 8);
   const int npairs = (h + 1) / 2;
+  fft_trace(ph, pw, P, CB);
   // algorithmic: read the real planes once, write the half spectrum once; ~2.5 N log2 N flops per real plane
   ProfScope ps("fft_rfft2", 2.5 * planes * (double)h * w * log2((double)h * w), 4.0 * planes * ((double)h * w + 2.0 * h * w2), st);
   rfft_rows_kernel<<<dim3((npairs + P - 1) / P, planes), 256, (size_t)2 * P * w * sizeof(float2), st>>>(src, tmp, h, w, w2, P, pw->dev);
@@ -264,6 +278,7 @@ void launch_irfft2(const View& spec, const View& out, const View* add, float2* t
   FftPlan* pw = fft_plan_get(w); FftPlan* ph = fft_plan_get(h);
   const int P = pick_batch(w, 8, 8), CB = pick_batch(h, 8, 8);
   const int npairs = (h + 1) / 2;
+  fft_trace(ph, pw, P, CB);
   ProfScope ps("fft_irfft2", 2.5 * planes * (double)h * w * log2((double)h * w),
                4.0 * planes * ((double)h * w * (add ? 2 : 1) + 2.0 * h * w2), st);
   fft_cols_kernel<<<dim3((w2 + CB - 1) / CB, planes), 256, (size_t)2 * CB * (h | 1) * sizeof(float2), st>>>(

@@ -425,6 +425,22 @@ bool use_tma_env() {
   if (v < 0) { const char* e = getenv("MITB_FFT_NO_TMA"); v = (e && atoi(e)) ? 0 : 1; }
   return v != 0;
 }
+// a pass may stage its tiles with the TMA box: neither MITB_FFT_NO_TMA nor the test hook's force_plain turned it off
+bool tma_allowed() { return use_tma_env() && !g_fft_force_plain; }
+
+void trace_plans(const FftNDev& ph, const FftNDev& pw) {
+  if (!g_fft_trace) return;
+  FftTrace& t = *g_fft_trace;
+  t = FftTrace();
+  t.h_nst = ph.nst; t.w_nst = pw.nst;
+  for (int s = 0; s < ph.nst; ++s) t.h_radix[s] = ph.radix[s];
+  for (int s = 0; s < pw.nst; ++s) t.w_radix[s] = pw.radix[s];
+}
+void trace_pass(bool rows, const FftKParams& p) {
+  if (!g_fft_trace) return;
+  (rows ? g_fft_trace->rows_tma : g_fft_trace->cols_tma) = p.use_tma ? 1 : 0;
+  (rows ? g_fft_trace->rows_box_rows : g_fft_trace->cols_box_rows) = p.use_tma ? p.box_rows : 0;
+}
 
 template <class K>
 void set_attr(K kernel, PerDeviceOnce& once) {
@@ -432,6 +448,8 @@ void set_attr(K kernel, PerDeviceOnce& once) {
 }
 
 }  // namespace
+
+bool g_fft_force_plain = false;
 
 bool fft_nhwc_supported(int h, int w, int C) {
   int radix[kMaxSt], nst;
@@ -452,10 +470,12 @@ void launch_rfft2_nhwc(const View& in, const SplitView* spec_sv, float* spec_f, 
   ProfScope ps("fft_rfft2", 2.5 * N * C * (double)h * w * log2((double)h * w), 4.0 * N * C * ((double)h * w + 2.0 * h * w2), st);
   FftKParams p; memset(&p, 0, sizeof(p));
   p.N = N; p.h = h; p.w = w; p.w2 = w2; p.C = C;
+  trace_plans(plan_get(h)->dev, plan_get(w)->dev);
   // rows
   p.pl = plan_get(w)->dev; p.in = in.p; p.in_cs = in.cs; p.in_coff = in.coff; p.out_f = reinterpret_cast<float*>(T);
   p.box_rows = box_rows_for(w);
-  p.use_tma = use_tma_env() && C % (2 * FV) == 0 && make_tile_map(&p.tmap, in.p, (long)N * h * w, in.cs, in.cs, p.box_rows);
+  p.use_tma = tma_allowed() && C % (2 * FV) == 0 && make_tile_map(&p.tmap, in.p, (long)N * h * w, in.cs, in.cs, p.box_rows);
+  trace_pass(true, p);
   rfft_rows_nhwc_kernel<<<dim3(N * h, (C / 2 + FV - 1) / FV), FT, smem_for(w), st>>>(p);
   count_launch();
   // cols
@@ -465,7 +485,8 @@ void launch_rfft2_nhwc(const View& in, const SplitView* spec_sv, float* spec_f, 
   MITB_CHECK(p.out_f || p.out_hi, "rfft2_nhwc: no output");
   p.scale = (float)(1.0 / sqrt((double)h * (double)w));
   p.box_rows = box_rows_for(h);
-  p.use_tma = use_tma_env() && C % FV == 0 && make_tile_map(&p.tmap, p.in, (long)N * h, (long)w2 * 2 * C, (long)w2 * 2 * C, p.box_rows);
+  p.use_tma = tma_allowed() && C % FV == 0 && make_tile_map(&p.tmap, p.in, (long)N * h, (long)w2 * 2 * C, (long)w2 * 2 * C, p.box_rows);
+  trace_pass(false, p);
   fft_cols_nhwc_kernel<false><<<dim3(N * w2, (C + FV - 1) / FV), FT, smem_for(h), st>>>(p);
   count_launch();
   CUDA_OK(cudaGetLastError());
@@ -484,11 +505,13 @@ void launch_irfft2_nhwc(const View& spec, const View& out, const SplitView* out_
   ProfScope ps("fft_irfft2", 2.5 * N * C * (double)h * w * log2((double)h * w), 4.0 * N * C * ((double)h * w * (add ? 2 : 1) + 2.0 * h * w2), st);
   FftKParams p; memset(&p, 0, sizeof(p));
   p.N = N; p.h = h; p.w = w; p.w2 = w2; p.C = C;
+  trace_plans(plan_get(h)->dev, plan_get(w)->dev);
   // cols (inverse): F -> T
   p.pl = plan_get(h)->dev; p.in = spec.p; p.in_cs = spec.cs; p.in_coff = spec.coff;
   p.out_f = reinterpret_cast<float*>(T); p.out_cs = 2 * C; p.out_coff = 0;
   p.box_rows = box_rows_for(h);
-  p.use_tma = use_tma_env() && C % FV == 0 && make_tile_map(&p.tmap, spec.p, (long)N * h, (long)w2 * spec.cs, (long)w2 * spec.cs, p.box_rows);
+  p.use_tma = tma_allowed() && C % FV == 0 && make_tile_map(&p.tmap, spec.p, (long)N * h, (long)w2 * spec.cs, (long)w2 * spec.cs, p.box_rows);
+  trace_pass(false, p);
   fft_cols_nhwc_kernel<true><<<dim3(N * w2, (C + FV - 1) / FV), FT, smem_for(h), st>>>(p);
   count_launch();
   // rows (inverse): T -> out
@@ -504,6 +527,7 @@ void launch_irfft2_nhwc(const View& spec, const View& out, const SplitView* out_
   p.add = add ? add->p : nullptr; p.add_cs = add ? add->cs : 0; p.add_coff = add ? add->coff : 0;
   p.scale = (float)(1.0 / sqrt((double)h * (double)w));
   p.use_tma = 0;
+  trace_pass(true, p);
   irfft_rows_nhwc_kernel<<<dim3(N * h, (C / 2 + FV - 1) / FV), FT, smem_for(w), st>>>(p);
   count_launch();
   CUDA_OK(cudaGetLastError());

@@ -252,6 +252,14 @@ void launch_irfft2(const View& spec, const View& out, const View* add /*planar, 
 bool fft_nhwc_supported(int h, int w, int C);
 void launch_rfft2_nhwc(const View& in, const SplitView* spec_sv, float* spec_f, float2* T, cudaStream_t st);
 void launch_irfft2_nhwc(const View& spec, const View& out, const SplitView* out_sv, int sv_coff, const View* add, float2* T, cudaStream_t st);
+// Host-side record of what the last FFT launch ran (test hook mitb_test_fft): null by default, and nothing is recorded then.
+// tma / box_rows: -1 on the planar path; P / CB: 0 on the NHWC path.
+struct FftTrace {
+  int h_nst = 0, h_radix[16] = {0}, w_nst = 0, w_radix[16] = {0};
+  int rows_tma = -1, rows_box_rows = -1, cols_tma = -1, cols_box_rows = -1, P = 0, CB = 0;
+};
+extern FftTrace* g_fft_trace;
+extern bool g_fft_force_plain;         // NHWC FFT: plain loads wherever the TMA box would run (test hook only)
 
 // ------------------------------------------------------------------ weights
 struct Weights {

@@ -1,7 +1,7 @@
 // Test hooks of include/mitb.h (not for production use): one fully described convolution through launch_conv(), so that tests
 // can reach every option of the fused conv epilogue (ConvOp in mitb_internal.h) on every kernel path and compare it with an
-// independent reference, and the OCR's vocabulary head (GEMM + fused log-softmax / argmax) with its row-stat partials.  Host
-// code only: the kernels are the ones the networks run.
+// independent reference, the OCR's vocabulary head (GEMM + fused log-softmax / argmax) with its row-stat partials, and one
+// real 2-D FFT on either FFT implementation.  Host code only: the kernels are the ones the networks run.
 #include <stddef.h>
 #include <string.h>
 #include "exec.h"
@@ -26,12 +26,22 @@ static_assert(offsetof(mitb_test_conv_info, bn) == 4 && offsetof(mitb_test_conv_
               offsetof(mitb_test_conv_info, convs) == 24 && offsetof(mitb_test_conv_info, staged) == 28 &&
               offsetof(mitb_test_conv_info, epi_sig) == 32 && sizeof(mitb_test_conv_info) == 36, "test hook info layout");
 
+static_assert(offsetof(mitb_test_fft_desc, N) == 8 && offsetof(mitb_test_fft_desc, in) == 24 && offsetof(mitb_test_fft_desc, out) == 48 &&
+              offsetof(mitb_test_fft_desc, out_sv) == 72 && offsetof(mitb_test_fft_desc, add) == 112 &&
+              offsetof(mitb_test_fft_desc, force_plain) == 136 && sizeof(mitb_test_fft_desc) == 144, "test hook fft descriptor layout");
+static_assert(offsetof(mitb_test_fft_info, h_radix) == 4 && offsetof(mitb_test_fft_info, w_nst) == 68 && offsetof(mitb_test_fft_info, w_radix) == 72 &&
+              offsetof(mitb_test_fft_info, rows_tma) == 136 && offsetof(mitb_test_fft_info, cols_tma) == 144 &&
+              offsetof(mitb_test_fft_info, P) == 152 && sizeof(mitb_test_fft_info) == 160, "test hook fft info layout");
+
 namespace {
 
-// restores the process-wide kernel switches and the trace / N tile overrides, also when the conv throws
+// restores the process-wide kernel switches and the trace / N tile / plain-load overrides, also when the call throws
 struct HookGuard {
   bool tc = conv_tc_enabled(), tma = conv_tma_enabled();
-  ~HookGuard() { conv_tc_set_enabled(tc); conv_tma_set_enabled(tma); g_conv_trace = nullptr; g_conv_force_bn = 0; }
+  ~HookGuard() {
+    conv_tc_set_enabled(tc); conv_tma_set_enabled(tma); g_conv_trace = nullptr; g_conv_force_bn = 0;
+    g_fft_trace = nullptr; g_fft_force_plain = false;
+  }
 };
 
 // the process-wide kernel switches of a MITB_TEST_PATH_*
@@ -219,6 +229,70 @@ int mitb_test_vocab_head(mitb_ctx* ctx, const float* x, int n, int t, int c, con
     MITB_CHECK(path != MITB_TEST_PATH_TMA || on_tma, "test_vocab_head: the op did not run on the TMA-fed kernel (kernel %d)", tr.kernel);
     fill_info(info, tr);
     *nblk = nb;
+    return 0;
+  } catch (const std::exception& ex) {
+    ctx->c.err = ex.what();
+    cudaGetLastError();
+    return 2;
+  }
+}
+
+int mitb_test_fft(mitb_ctx* ctx, const mitb_test_fft_desc* d, mitb_test_fft_info* info, void* stream) {
+  if (!ctx) return 1;
+  HookGuard guard;
+  try {
+    CUDA_OK(cudaSetDevice(ctx->c.device));
+    MITB_CHECK(d && info, "test_fft: null descriptor or info");
+    cudaStream_t st = (cudaStream_t)stream;
+    MITB_CHECK(d->impl == MITB_TEST_FFT_PLANAR || d->impl == MITB_TEST_FFT_NHWC, "test_fft: bad implementation %d", d->impl);
+    MITB_CHECK(d->N > 0 && d->h > 0 && d->w > 0 && d->C > 0, "test_fft: bad shape");
+    MITB_CHECK(d->in.p, "test_fft: no input");
+    const bool nhwc = d->impl == MITB_TEST_FFT_NHWC, inv = d->inverse != 0;
+    const int N = d->N, h = d->h, w = d->w, C = d->C, w2 = w / 2 + 1;
+    const int cin = inv ? 2 * C : C, cout = inv ? C : 2 * C;      // channels of the input / output views
+    const void* al16[] = {d->in.p, d->out.p, d->add.p, d->out_sv.hi, d->out_sv.mid};
+    const char* al16_name[] = {"in", "out", "add", "out_sv.hi", "out_sv.mid"};
+    for (int i = 0; i < 5; ++i) check_align(al16[i], 16, al16_name[i]);
+    // a view of channels [coff, coff + c) of [N][H][W][cs] (planar: contiguous planes)
+    auto view = [&](const mitb_test_view& v, int H, int W, int c) {
+      View r; r.p = (float*)v.p; r.N = N; r.H = H; r.W = W; r.C = c; r.planar = !nhwc;
+      r.cs = nhwc ? v.cs : c; r.coff = nhwc ? v.coff : 0;
+      MITB_CHECK(!v.p || nhwc || ((v.cs == 0 || v.cs == c) && v.coff == 0), "test_fft: planar views are contiguous planes");
+      MITB_CHECK(!v.p || (r.cs > 0 && r.coff >= 0 && r.coff + c <= r.cs), "test_fft: slice [%d, %d) outside cs %d", r.coff, r.coff + c, r.cs);
+      return r;
+    };
+    const View in = view(d->in, h, inv ? w2 : w, cin);
+    const View out = view(d->out, h, inv ? w : w2, cout);
+    MITB_CHECK(!d->add.p || inv, "test_fft: the residual belongs to the inverse");
+    const View add = view(d->add, h, w, C);
+    MITB_CHECK(!d->out_sv.hi || nhwc, "test_fft: the split output exists on the NHWC path only");
+    MITB_CHECK(!d->force_plain || nhwc, "test_fft: force_plain is an NHWC switch");
+    MITB_CHECK(d->out.p || d->out_sv.hi, "test_fft: no output");
+    SplitView sv;
+    if (d->out_sv.hi) {
+      MITB_CHECK(d->out_sv.mid && d->out_sv.pt == 0 && d->out_sv.pl == 0, "test_fft: split output without mid or with a halo");
+      sv.hi = d->out_sv.hi; sv.mid = d->out_sv.mid; sv.N = N; sv.H = h; sv.W = inv ? w : w2; sv.C = d->out_sv.C;
+      sv.Hp = d->out_sv.Hp; sv.Wp = d->out_sv.Wp;
+      MITB_CHECK(inv || d->out_sv.coff == 0, "test_fft: the forward split output is dense");
+    }
+    MITB_CHECK(inv || !nhwc || !d->out.p || (d->out.cs == 2 * C && d->out.coff == 0), "test_fft: the forward fp32 output is dense");
+
+    DevBlob blob;
+    float2* tmp = (float2*)blob.alloc_f((size_t)2 * N * C * h * w2);
+    FftTrace tr;
+    g_fft_trace = &tr; g_fft_force_plain = d->force_plain != 0;
+    CUDA_OK(cudaStreamSynchronize(st));
+    ++g_launch_epoch;
+    if (!nhwc && !inv) launch_rfft2(in, out, tmp, st);
+    else if (!nhwc) launch_irfft2(in, out, add.p ? &add : nullptr, tmp, st);
+    else if (!inv) launch_rfft2_nhwc(in, sv.valid() ? &sv : nullptr, out.p, tmp, st);
+    else launch_irfft2_nhwc(in, out, sv.valid() ? &sv : nullptr, d->out_sv.coff, add.p ? &add : nullptr, tmp, st);
+    CUDA_OK(cudaStreamSynchronize(st));
+    memset(info, 0, sizeof(*info));
+    info->h_nst = tr.h_nst; info->w_nst = tr.w_nst;
+    for (int s = 0; s < 16; ++s) { info->h_radix[s] = tr.h_radix[s]; info->w_radix[s] = tr.w_radix[s]; }
+    info->rows_tma = tr.rows_tma; info->rows_box_rows = tr.rows_box_rows; info->cols_tma = tr.cols_tma; info->cols_box_rows = tr.cols_box_rows;
+    info->P = tr.P; info->CB = tr.CB;
     return 0;
   } catch (const std::exception& ex) {
     ctx->c.err = ex.what();

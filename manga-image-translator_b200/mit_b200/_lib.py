@@ -47,6 +47,17 @@ class MitbTestConvInfo(C.Structure):
     _fields_ = _ints("kernel", "bn", "splits", "vec2", "tma_act", "split_reused", "convs", "staged", "epi_sig")
 
 
+class MitbTestFftDesc(C.Structure):
+    """mitb_test_fft_desc (test hook, include/mitb.h): one real 2-D FFT on the planar or the NHWC implementation."""
+    _fields_ = (_ints("impl", "inverse", "N", "h", "w", "C") + [("in", MitbTestView), ("out", MitbTestView), ("out_sv", MitbTestSplit),
+                                                                ("add", MitbTestView)] + _ints("force_plain", "reserved"))
+
+
+class MitbTestFftInfo(C.Structure):
+    _fields_ = ([("h_nst", C.c_int32), ("h_radix", C.c_int32 * 16), ("w_nst", C.c_int32), ("w_radix", C.c_int32 * 16)] +
+                _ints("rows_tma", "rows_box_rows", "cols_tma", "cols_box_rows", "P", "CB"))
+
+
 class MitbError(RuntimeError):
     pass
 
@@ -111,6 +122,7 @@ SIGNATURES = {
     "mitb_test_conv": (I, [P, C.POINTER(MitbTestConvDesc), C.POINTER(MitbTestConvInfo), P]),
     "mitb_test_struct_sizes": (I, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "mitb_test_vocab_head": (I, [P, P, I, I, I, P, P, I, I, P, P, P, P, P, LL, C.POINTER(C.c_int32), C.POINTER(MitbTestConvInfo), P]),
+    "mitb_test_fft": (I, [P, C.POINTER(MitbTestFftDesc), C.POINTER(MitbTestFftInfo), P]),
     "mitb_set_epi_specialise": (I, [I]),
     "mitb_test_epi_signature": (I, [I, I]),
     "mitb_test_epi_signatures": (I, [C.POINTER(C.c_int), C.POINTER(C.c_int), I]),

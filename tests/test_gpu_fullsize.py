@@ -3,6 +3,7 @@ the CPU oracle run on this box's host cores:
 
   * DBNetConvNext.forward on one 2048x1536 page          (dbnet_convnext.py:474-491)   db, mask <= 1e-3, IoU >= 0.999
   * LamaFourier (MPE, 9 blocks) on one 2048x1536 page    (inpainting_lama_mpe.py:713-726)   <= 1e-3
+  * the same on a 1448x2048 page (an A4 scan): bottleneck 181x256, the planar FFT with its prime-radix stage   <= 1e-3
   * OCR.decode front half on one 16x48x647 chunk, V=46000 (model_48px_ctc.py:447-463)   argmax identical where the oracle's
     top-2 margin exceeds 1e-3, and the number of excluded steps is bounded
   * lama_large (18 blocks) on one 2560x1920 page = --inpainting-size 2560 (inpainting_lama_mpe.py:121-136; FFT 320x240)
@@ -99,6 +100,31 @@ def test_lama_mpe_2048x1536(eng):
     _record("lama_mpe_2048x1536", max_abs=e, mean_abs_in_hole=(out - o).abs()[inside].mean().item(), oracle_s=time.time() - t0)
     assert e < TOL
     assert torch.equal(out[~inside], img[~inside])      # untouched outside the hole (inpainting_lama_mpe.py:726)
+
+
+def test_lama_mpe_1448x2048_planar_fft(eng):
+    """An A4 scan at a 2048 px long side: the bottleneck is 181 x 256 and 181 is prime, so every FFC layer runs the planar FFT
+    (fft.cu) with its generic prime-radix stage.  Forcing the planar FFC path (mode 0) gives the same bits as the default mode,
+    which shows that the planar path is the one the default mode ran."""
+    sd, msd = weights.lama_weights(9), weights.mpe_weights()
+    img, mask = _lama_page(1448, 2048, 1448)
+    rel, direct = nets.mpe_tables(mask[0, 0].numpy())
+    eng.load_lama(sd, msd)
+    try:
+        out = eng.lama_forward(img, mask, rel[None], direct[None]).cpu()
+        eng.set_ffc_mode(0)
+        out0 = eng.lama_forward(img, mask, rel[None], direct[None]).cpu()
+    finally:
+        eng.set_ffc_mode(1)
+        eng.unload_lama()
+    assert torch.equal(out, out0), "default FFC mode differs from the planar path at a 181 x 256 bottleneck"
+    t0 = time.time()
+    o = nets.lama_forward(sd, msd, img, mask, torch.from_numpy(rel)[None], torch.from_numpy(direct)[None])
+    e = (out - o).abs().max().item()
+    inside = (mask > 0).expand_as(out)
+    _record("lama_mpe_1448x2048", max_abs=e, mean_abs_in_hole=(out - o).abs()[inside].mean().item(), oracle_s=time.time() - t0)
+    assert e < TOL
+    assert torch.equal(out[~inside], img[~inside])
 
 
 def test_ocr_chunk_16x48x647_v46000(eng):

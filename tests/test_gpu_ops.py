@@ -102,53 +102,6 @@ def test_layernorm(eng, c):
     _close(eng.layernorm(x, w, b, 1e-5), F.layer_norm(x, (c,), w, b, 1e-5), what=f"layernorm {c}")
 
 
-FFT_SIZES = [(8, 8), (16, 12), (20, 14), (11, 15), (32, 24), (256, 192), (40, 30), (97, 6), (6, 97), (13, 128)]
-
-
-@pytest.mark.parametrize("h,w", FFT_SIZES)
-def test_rfft2_irfft2(eng, h, w):
-    g = torch.Generator().manual_seed(h * 1000 + w)
-    c = 3 if h * w > 10000 else 6
-    x = torch.randn(c, h, w, generator=g)
-    f = torch.fft.rfftn(x, dim=(-2, -1), norm="ortho")
-    ref = torch.stack((f.real, f.imag), dim=1).reshape(2 * c, h, w // 2 + 1)
-    spec = eng.rfft2(x)
-    _close(spec, ref, 2e-5, what=f"rfft2 {h}x{w}")
-    # inverse of an arbitrary (non-Hermitian-consistent) half spectrum, like the one after conv+ReLU
-    s = torch.randn(2 * c, h, w // 2 + 1, generator=g)
-    z = torch.complex(s.view(c, 2, h, -1)[:, 0].contiguous(), s.view(c, 2, h, -1)[:, 1].contiguous())
-    ref = torch.fft.irfftn(z, s=(h, w), dim=(-2, -1), norm="ortho")
-    _close(eng.irfft2(s, w), ref, 2e-5, what=f"irfft2 {h}x{w}")
-
-
-@pytest.mark.parametrize("n,h,w,c", [(1, 16, 12, 64), (2, 8, 8, 2), (1, 20, 30, 6), (1, 256, 192, 64), (1, 320, 240, 64), (2, 32, 24, 192),
-                                     (1, 5, 9, 70), (1, 64, 50, 34)])
-def test_rfft2_irfft2_nhwc(eng, n, h, w, c):
-    """Channel-vectorised NHWC FFT (fft_nhwc.cu) against torch.fft, incl. channel counts that are not multiples of the 32-lane
-    chunk (plain-load path instead of the TMA box), odd widths and the 256x192 / 320x240 sizes of the bench configs."""
-    g = torch.Generator().manual_seed(n * 7 + h * 1000 + w + c)
-    x = torch.randn(n, h, w, c, generator=g)
-    f = torch.fft.rfftn(x.permute(0, 3, 1, 2), dim=(-2, -1), norm="ortho")                  # [n,c,h,w2]
-    ref = torch.stack((f.real, f.imag), dim=2).permute(0, 3, 4, 1, 2).reshape(n, h, w // 2 + 1, 2 * c)
-    _close(eng.rfft2_nhwc(x), ref, 2e-5, what=f"rfft2_nhwc {h}x{w}x{c}")
-    s = torch.randn(n, h, w // 2 + 1, 2 * c, generator=g)
-    add = torch.randn(n, h, w, c, generator=g)
-    sc = s.view(n, h, w // 2 + 1, c, 2).permute(0, 3, 1, 2, 4)
-    z = torch.complex(sc[..., 0].contiguous(), sc[..., 1].contiguous())
-    ref = torch.fft.irfftn(z, s=(h, w), dim=(-2, -1), norm="ortho").permute(0, 2, 3, 1)
-    _close(eng.irfft2_nhwc(s, w), ref, 2e-5, what=f"irfft2_nhwc {h}x{w}x{c}")
-    _close(eng.irfft2_nhwc(s, w, add), ref + add, 2e-5, what=f"irfft2_nhwc+add {h}x{w}x{c}")
-
-
-def test_fft_impulse_and_roundtrip(eng):
-    x = torch.zeros(2, 24, 20)
-    x[0, 0, 0] = 1.0
-    x[1, 5, 7] = 2.0
-    spec = eng.rfft2(x).cpu()
-    assert (spec[0] - 1 / (24 * 20) ** 0.5).abs().max() < 1e-6 and spec[1].abs().max() < 1e-6   # flat real spectrum
-    _close(eng.irfft2(spec, 20), x, 2e-6, what="fft round trip")
-
-
 def test_mpe_tables_device_equals_host(eng):
     """The device distance / direction sweep (mitb_op_mpe_tables) is bit-identical to the host restatement of
     load_masked_position_encoding (inpainting_lama_mpe.py:751-815), incl. the degenerate all-hole / no-hole masks."""

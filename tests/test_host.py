@@ -32,7 +32,7 @@ def test_abi_header_and_library_agree():
 
 
 def test_test_hook_structs_match_header():
-    """The ctypes mirrors of the conv test hook's structs have the library's sizes and the field offsets include/mitb.h states
+    """The ctypes mirrors of the conv and FFT test hooks' structs have the library's sizes and the field offsets include/mitb.h states
     ("@N" on a field's line is the offset of the first field declared there; "N bytes" after a struct is its size)."""
     from mit_b200 import _lib
     lib = _lib.load()
@@ -41,7 +41,8 @@ def test_test_hook_structs_match_header():
     assert (d.value, i.value) == (ctypes.sizeof(_lib.MitbTestConvDesc), ctypes.sizeof(_lib.MitbTestConvInfo))
     hdr = open(os.path.join(ROOT, "include", "mitb.h")).read()
     mirrors = {"mitb_test_view": _lib.MitbTestView, "mitb_test_split": _lib.MitbTestSplit,
-               "mitb_test_conv_desc": _lib.MitbTestConvDesc, "mitb_test_conv_info": _lib.MitbTestConvInfo}
+               "mitb_test_conv_desc": _lib.MitbTestConvDesc, "mitb_test_conv_info": _lib.MitbTestConvInfo,
+               "mitb_test_fft_desc": _lib.MitbTestFftDesc, "mitb_test_fft_info": _lib.MitbTestFftInfo}
     stated = 0
     for name, mirror in mirrors.items():
         body, size = re.search(r"typedef struct \{([^{}]*)\}\s*" + name + r";\s*/\*\s*(\d+) bytes", hdr, re.S).groups()
@@ -56,7 +57,7 @@ def test_test_hook_structs_match_header():
                 assert getattr(mirror, fields[0]).offset == int(m.group(1)), (name, fields[0])
                 stated += 1
         assert declared == [f[0] for f in mirror._fields_], name      # same fields in the same order
-    assert stated >= 25
+    assert stated >= 38
 
 
 def test_no_cpu_fallback():
